@@ -54,6 +54,9 @@ def parse():
     ap.add_argument("--no-shim-leg", action="store_true", help="skip the reference-host-with-GPU-shim point (64 files through oracle/_ref/jref_gpu)")
     ap.add_argument("--no-extra-legs", action="store_true", help="skip the 1-utterance / 16-utterance points and the short DNN-HMM leg")
     ap.add_argument("--cpu-sample-utts", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (pass-1 best and, for a fixed sample of utterances, the word "
+                         "trellis) as DIR/<name>.npy, so that two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -107,23 +110,12 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def kernel_source_sha() -> str:
-    """identity of the CUDA sources a committed ncu capture belongs to"""
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "julius_b200", "csrc")
-    for fn in sorted(os.listdir(d)):
-        if fn.endswith((".cu", ".cuh", ".inc")):
-            h.update(open(os.path.join(d, fn), "rb").read())
-    return h.hexdigest()[:16]
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # --------------------------------------------------------------------------------------- reference arm
@@ -163,8 +155,7 @@ def host_cpus() -> dict:
 
 def ref_procs(info: dict | None = None) -> int:
     """One reference process per physical core this process may use: the decoder is single-threaded and
-    memory-bound, one per hardware thread is slower in aggregate (measured on a B200 box: 64 processes
-    6.2k frames/s, 128 processes 3.5k frames/s).  JB200_REF_PROCS overrides."""
+    memory-bound, and two processes sharing a core's hardware threads are slower in aggregate.  JB200_REF_PROCS overrides."""
     if os.environ.get("JB200_REF_PROCS"):
         return max(1, int(os.environ["JB200_REF_PROCS"]))
     info = info or host_cpus()
@@ -308,24 +299,46 @@ def workload_label(name: str) -> str:
 
 # --------------------------------------------------------------------------------------- product arm
 def fp32_peak():
-    """FP32 SIMT peak for the GMM scoring roofline: measured by tools/ubench/ffma.cu (profiles/fp32_peak.json) when that
-    capture exists, else the nominal 148 SM x 128 lanes x 2 flop x max SM clock."""
-    p = os.path.join(ROOT, "profiles", "fp32_peak.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return float(d["ffma_tflops"]), f"measured FFMA micro-benchmark (profiles/fp32_peak.json, {d.get('when', '')})"
-    return 148 * 128 * 2 * 1.965e9 / 1e12, "nominal 148 SM x 128 lanes x 2 x 1.965 GHz (no measured FP32 figure in MEASURED_PEAKS.json)"
+    """FP32 SIMT peak for the GMM scoring roofline: the H100 SXM data sheet's dense FP32 rate (132 SMs x 128 lanes x 2 flop
+    at the boost clock).  A power-limited card reaches less."""
+    return 67.0, "H100 SXM data sheet, dense FP32 (67 TFLOP/s), not measured"
 
 
-# frames per time slice of the batch pipeline for GMM workloads (DESIGN.md section 4, "batch pipeline"): measured on tri20k,
-# 444 utterances (profiles/exp_r02_slices.txt): 1.391 M frames/s with 96-frame slices, 1.432 M with 64, 1.430 M with 48,
-# 1.446 M with 32 (one launch per batch at 592 utterances: 1.357 M)
+# frames per time slice of the batch pipeline for GMM workloads (DESIGN.md section 4, "batch pipeline")
 PIPE_FRAMES_DEFAULT = 32
 
 
-def measure_workload(ctx, name, B, T, steps, warmup, mode="exact", want_e2e=True, n_batches=2, seed0=100, pipe_frames=0):
+DUMP_SAMPLE_UTTS = 16                  # utterances whose full word trellis --dump-outputs writes
+DUMP_MAX_BYTES = 48 << 20
+
+
+def dump_outputs(res, out_dir: str) -> None:
+    """The results of one batch as float64 arrays: per utterance (status, overflow, frames, atoms, score) and the pass-1
+    best word ids (-1 padded) for all utterances; the word trellis (utterance, wid, begin, end, backscore, lscore, last)
+    of a fixed seeded sample of utterances, as many of them as fit in DUMP_MAX_BYTES."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(res)
+    info = np.array([[r["status"], r["overflow"], r["n_frames"], len(r["atoms"]), r["score"]] for r in res], np.float64).reshape(n, 5)
+    words = np.full((n, max([len(r["words"]) for r in res] + [1])), -1.0)
+    for i, r in enumerate(res):
+        words[i, :len(r["words"])] = r["words"]
+    sample = np.sort(np.random.default_rng(0).choice(n, min(n, DUMP_SAMPLE_UTTS), replace=False))
+    rows, nbytes = [], 0
+    for i in sample:
+        a = res[i]["atoms"]
+        if nbytes + len(a) * 7 * 8 > DUMP_MAX_BYTES:
+            break
+        rows.append(np.stack([np.full(len(a), i), a["wid"], a["begin"], a["end"], a["backscore"], a["lscore"], a["last"]], 1).astype(np.float64))
+        nbytes += len(a) * 7 * 8
+    np.save(os.path.join(out_dir, "utterances.npy"), info)
+    np.save(os.path.join(out_dir, "best_words.npy"), words)
+    np.save(os.path.join(out_dir, "trellis_sample.npy"), np.concatenate(rows, 0) if rows else np.zeros((0, 7)))
+
+
+def measure_workload(ctx, name, B, T, steps, warmup, mode="exact", want_e2e=True, n_batches=2, seed0=100, pipe_frames=0,
+                     dump_dir=None):
     """W warm-up + K timed steps of one workload at B utterances x T frames per GPU; returns the measured figures.
-    ctx: dict(rank, local, world, device, torch, dist)."""
+    ctx: dict(rank, local, world, device, torch, dist).  dump_dir: write the last timed step's results there (rank 0)."""
     torch, dist = ctx["torch"], ctx["dist"]
     from julius_b200 import capi, desc, workload
     from julius_b200.dist import broadcast_blob
@@ -348,9 +361,8 @@ def measure_workload(ctx, name, B, T, steps, warmup, mode="exact", want_e2e=True
     probe = capi.Decoder(ds, am, max_utts=1, max_frames=8)
     resident = max(1, probe.resident_utts())       # one resident wave of thread blocks
     probe.close()
-    # the pipeline pays off where a K1 block beside three beam blocks beats a fourth beam block: GMM scoring on normal trees
-    # (measured: tri20k +7 %, tri20k_gbeam +29 %; the multipath kernel loses more from the missing block than the overlap
-    # returns: tri20k_mp 0.69 M sliced at 444 utterances against 0.79 M unsliced at 592)
+    # the pipeline is meant for where a K1 block beside three beam blocks beats a fourth beam block: GMM scoring on normal
+    # trees; the multipath kernel loses more from the missing block than the overlap returns
     pipe = 0 if (use_dnn or int(ds.tree.multipath)) else max(0, pipe_frames)
     if not B:
         # the pipeline needs room for one scoring thread block beside the beam's on every SM: 3/4 of a resident wave
@@ -413,6 +425,9 @@ def measure_workload(ctx, name, B, T, steps, warmup, mode="exact", want_e2e=True
     dev_ms = sum(score_ms) + sum(beam_ms)
     barrier()
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
+    if dump_dir and rank == 0:
+        dec._last_n = B
+        dump_outputs(dec.results(), dump_dir)
 
     # ---------------- e2e: host buffers through the C-ABI ----------------
     e2e_ms = h2d = d2h = 0
@@ -471,27 +486,14 @@ def rooflines(r, world):
     gmm_bytes = r["M_total"] * ALG_GMM_BYTES_PER_GAUSS + B * T * (r["D"] * 4 + 4 * S)
     beam_bytes = B * T * r["tokens_per_frame"] * ALG_BEAM_BYTES_PER_TOKEN
     beam_name = "beam_kernel_mp" if r["multipath"] else "beam_kernel"
-    score_name = "dnn_gemm_persistent (x%d layers)" % r["dnn_layers"] if r["use_dnn"] else "gmm_score_kernel"
+    score_name = "dnn_gemm_wgmma (x%d layers)" % r["dnn_layers"] if r["use_dnn"] else "gmm_score_kernel"
     if bm_ms >= gmm_ms:
         dom, dom_ms, dom_bytes = beam_name, bm_ms, beam_bytes
     else:
         dom, dom_ms, dom_bytes = score_name, gmm_ms, gmm_bytes
     ach = dom_bytes / (dom_ms / 1000.0) / 1e9
-    traffic, traffic_note = None, "no ncu capture of this kernel build under profiles/"
-    tfile = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tfile):
-        tj = json.load(open(tfile))
-        ent = tj.get(dom)
-        if ent is not None and ent.get("source_sha") != kernel_source_sha():
-            traffic_note = (f"profiles/ncu_traffic.json was captured from another build of {dom} "
-                            f"(source_sha {ent.get('source_sha')} != {kernel_source_sha()}): not reported")
-        elif ent is not None:
-            per = ent.get("bytes_per_utterance_frame", ent.get("bytes_per_frame"))
-            traffic = per * B * T
-            traffic_note = f"ncu dram read+write of this build ({ent.get('capture')}), per utterance-frame x {B * T} utterance-frames"
     hs = r["heap"]
     roof = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-            "traffic": traffic, "traffic_unit": "bytes per launch", "traffic_note": traffic_note,
             "algorithmic_bytes": dom_bytes, "peak_source": peak_src,
             "kernel_ms": {score_name: gmm_ms, beam_name: bm_ms},
             "pipeline": ({"slices": r["pipe_slices"], "frames_per_slice": r["pipe_frames"], "scoring_exposed_ms": r["score_ms"],
@@ -508,13 +510,13 @@ def rooflines(r, world):
                          "replay_ticks_per_extraction": round(hs["levels"] / max(hs["extractions"], 1), 3)}}
     if r["use_dnn"]:
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-        tpeak = float(pk.get("bf16_tflops_sustained", 1400.0))
+        tpeak = float(pk.get("bf16_tflops_sustained", 989.0))
         tach = B * T * r["dnn_flops_per_frame"] / (gmm_ms / 1000.0) / 1e12
         scoring = {"bound": "tensor", "kernel": score_name, "achieved": tach, "peak": tpeak, "unit": "TFLOP/s", "frac": tach / tpeak,
                    "ms": gmm_ms, "frames_per_s": B * T / (gmm_ms / 1000.0),
                    "note": "algorithmic flops (2*in*out per layer per frame); the kernel issues 3 bf16 MMAs per product term "
                            "(hi.hi+hi.lo+lo.hi) to meet the 1e-4 tolerance, so 1/3 of peak is the ceiling of this formulation",
-                   "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if pk else "fallback 1.4 PFLOP/s sustained"}
+                   "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if pk else "H100 SXM data sheet, dense BF16 (989 TFLOP/s), not measured"}
     else:
         fpeak, fsrc = fp32_peak()
         fach = B * T * r["M_total"] * ALG_FLOPS_PER_GAUSS_FRAME / (gmm_ms / 1000.0) / 1e12
@@ -522,7 +524,7 @@ def rooflines(r, world):
                    "ms": gmm_ms, "frames_per_s": B * T / (gmm_ms / 1000.0), "hbm_gbs": gmm_bytes / (gmm_ms / 1000.0) / 1e9,
                    "hbm_frac": gmm_bytes / (gmm_ms / 1000.0) / 1e9 / peak,
                    "note": "algorithmic flops (162 per Gaussian-frame, SURVEY 8d); a parameter record is reused for 256 frames, so the "
-                           "batch kernel is FP32-issue bound, not HBM bound (ridge ~10 flop/B)",
+                           "batch kernel is FP32-issue bound, not HBM bound (ridge ~20 flop/B on an H100)",
                    "peak_source": fsrc}
     return roof, scoring
 
@@ -596,7 +598,7 @@ def product_main(a):
     ctx = dict(rank=rank, local=local, world=world, device=device, torch=torch, dist=dist)
 
     pf = PIPE_FRAMES_DEFAULT if a.pipe_frames < 0 else a.pipe_frames
-    r = measure_workload(ctx, a.workload, a.utts, a.frames, a.steps, a.warmup, mode=a.mode, pipe_frames=pf)
+    r = measure_workload(ctx, a.workload, a.utts, a.frames, a.steps, a.warmup, mode=a.mode, pipe_frames=pf, dump_dir=a.dump_outputs)
     B, T = r["B"], r["T"]
     extra = {}
     if world == 1 and not a.no_extra_legs:
@@ -622,7 +624,8 @@ def product_main(a):
         if a.workload != "dnn20k":
             from julius_b200 import workload as _w
             if _w.ready("dnn20k"):
-                q = measure_workload(ctx, "dnn20k", a.utts or min(r["resident"], 148), T, 2, 2, want_e2e=True)
+                q = measure_workload(ctx, "dnn20k", a.utts or min(r["resident"], torch.cuda.get_device_properties(device).multi_processor_count),
+                                     T, 2, 2, want_e2e=True)
                 qroof, qscoring = rooflines(q, world)
                 extra["dnn20k"] = {"config": {"workload": workload_label("dnn20k"), "utts_per_gpu": q["B"], "frames_per_utt": T},
                                    "value": q["B"] * T * q["steps"] / (q["wall_ms"] / 1000.0), "unit": "frames/s",

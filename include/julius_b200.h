@@ -1,4 +1,4 @@
-/* julius_b200.h -- C-ABI of libjb200.so: B200-native acoustic scoring + pass-1 beam for Julius.
+/* julius_b200.h -- C-ABI of libjb200.so: H100-native acoustic scoring + pass-1 beam for Julius.
  *
  * Plain C: pointers, sizes, opaque handles.  No torch / CUDA types.  Every
  * entry point names the reference interface it stands in for (file:line in
@@ -13,7 +13,7 @@
  *     handle's own stream).
  *   - scores are log10 likelihoods, exactly the values the reference keeps in
  *     HMMWork.outprob_cache[t][state-id] (libsent/include/sent/hmm_calc.h:115).
- *   - there is NO CPU fallback: creating a handle without a usable sm_100 GPU fails.
+ *   - there is NO CPU fallback: creating a handle without a usable sm_90 GPU fails.
  */
 #ifndef JULIUS_B200_H
 #define JULIUS_B200_H

@@ -1,4 +1,4 @@
-"""Build libjb200.so (CUDA, sm_100a only) in-tree with nvcc.  No JIT cache: the .so travels."""
+"""Build libjb200.so (CUDA, sm_90a only) in-tree with nvcc.  No JIT cache: the library is loaded from the tree."""
 from __future__ import annotations
 
 import glob
@@ -10,7 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libjb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*GENCODE, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -54,7 +55,7 @@ def build(force: bool = False, verbose: bool = False, variant: str = "", defines
         f.write("\n".join(log))
     if verbose:
         print("\n".join(log))
-    subprocess.run([NVCC, "-shared", "-o", lib, *objs, "-gencode", "arch=compute_100a,code=sm_100a"], check=True)
+    subprocess.run([NVCC, "-shared", "-o", lib, *objs, *GENCODE], check=True)
     return lib
 
 

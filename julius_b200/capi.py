@@ -1,6 +1,6 @@
 """ctypes binding of libjb200.so (include/julius_b200.h) -- the product's host-side mirror.
 
-Fails loudly when the CUDA library is missing or no B200 is visible: there is no CPU path here.
+Fails loudly when the CUDA library is missing or no H100 is visible: there is no CPU path here.
 """
 from __future__ import annotations
 

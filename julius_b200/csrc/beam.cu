@@ -2110,8 +2110,7 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
     d->resident = per_sm * sms;
   }
   // Opt-in (JB200_L2_WINDOW=1): an L2 access-policy window that keeps the shared tables resident (persisting hits, streaming
-  // misses).  Measured on the 20k-word workload with 592 distinct utterances: 1.194 M frames/s with the window, 1.224 M
-  // without -- the set-aside costs the per-utterance work areas more than it saves on tree / LM lines -- so it is off.
+  // misses).  Off by default: the set-aside competes with the per-utterance work areas for L2.
   if (d->arena && d->arena_used > 0 && getenv("JB200_L2_WINDOW") != nullptr && atoi(getenv("JB200_L2_WINDOW")) != 0) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, d->device) == cudaSuccess && prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {

@@ -1,4 +1,4 @@
-// dnn.cu -- K2: DNN-HMM forward for all frames of a batch on the 5th-generation tensor cores.
+// dnn.cu -- K2: DNN-HMM forward for all frames of a batch on the Hopper tensor cores (wgmma).
 //
 // Stands in for dnn_calc_outprob (libsent/src/phmm/calc_dnn.c:774-868): per frame a stack of
 //   dst = W.src + b   (calc_dnn_fma.c:18-95 / sub1 calc_dnn.c:509-523)
@@ -10,18 +10,20 @@
 // Precision.  The parity tolerance is 1e-4 relative on log-likelihoods; a single bf16/tf32 pass
 // (8/10-bit mantissa) is ~1e-3.  Every operand is therefore split in two bf16 terms
 // (x = hi + lo, 16 mantissa bits) and each k-block issues three MMAs into the same fp32
-// accumulator in TMEM:  hi.hi + hi.lo + lo.hi   (the dropped lo.lo term is 2^-16 relative).
+// register accumulator:  hi.hi + hi.lo + lo.hi   (the dropped lo.lo term is 2^-16 relative).
 //
-// Kernel anatomy (sm_100a), dnn_gemm_persistent<256> by default (dnn_gemm_kernel = the one-tile-per-CTA
-// first version, JB200_DNN_KERNEL=0): 192 threads = warp 0 TMA producer, warp 1 tcgen05.mma issuer,
-// warps 2-5 epilogue (each owns the TMEM lane quarter warp_idx%4).  Operand tiles
-// 128 x 64 bf16 (K-major, 128-byte swizzle) arrive by cp.async.bulk.tensor (TMA) into a 3-stage
-// shared-memory ring guarded by full/empty mbarriers; the 128 x 128 fp32 accumulator lives in
-// TMEM; tcgen05.commit hands stages back to the producer and the finished tile to the epilogue,
-// which reads it with tcgen05.ld, adds the bias, applies the reference's clamped table logistic and
-// writes the next layer's operands already split into bf16 hi/lo.  The last layer's epilogue
-// writes fp32 logits; a row kernel then does the log-softmax (with the reference's "drop terms more
-// than 13.8 below the sum" rule) and subtracts the log10 prior.
+// Kernel anatomy (sm_90a), dnn_gemm_wgmma: a persistent CTA per SM walks the 128 x 128 output tiles
+// (column blocks fastest, so the CTAs that run side by side share the activation rows in L2).
+// 384 threads = warpgroup 0 (one thread: the TMA producer) + two consumer warpgroups, each owning
+// 64 rows of the tile.  Operand tiles 128 x 64 bf16 (K-major, 128-byte swizzle) arrive by
+// cp.async.bulk.tensor (TMA) into a 3-stage shared-memory ring guarded by full/empty mbarriers
+// (3 x 64 KB of the 227 KB a block may have).  The consumers issue wgmma.mma_async m64n128k16 straight
+// from shared memory into 64 fp32 registers per thread, keep one wgmma group in flight while they
+// wait for the next stage, and then run the epilogue from registers: bias, the reference's clamped
+// table logistic, and the next layer's operands already split into bf16 hi/lo.  The producer runs
+// ahead into the next tile meanwhile.  The last layer's epilogue writes fp32 logits; a row kernel then
+// does the log-softmax (with the reference's "drop terms more than 13.8 below the sum" rule) and
+// subtracts the log10 prior.
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -33,7 +35,8 @@ namespace jb200 {
 static constexpr int BM = 128, BN = 128, BK = 64, STAGES = 3;
 static constexpr int TILE_BYTES = BM * BK * 2;                 // 16 KB (A and B tiles are the same size)
 static constexpr int STAGE_BYTES = 4 * TILE_BYTES;             // A_hi A_lo B_hi B_lo
-static constexpr int GEMM_THREADS = 192;
+static constexpr int CONSUMERS = 2;                            // warpgroups, 64 rows each
+static constexpr int GEMM_THREADS = 128 * (1 + CONSUMERS);
 static constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 static constexpr int LOGISTIC_N = 320001;
 
@@ -45,40 +48,26 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               :: "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// K-major, 128-byte swizzle operand descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 [0,14) | LBO=1 [16,30) | SBO=1024>>4 [32,46) | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
+// K-major, 128-byte swizzle wgmma matrix descriptor: start>>4 [0,14) | LBO=1 [16,30) (unused with this swizzle) |
+// SBO=1024>>4 [32,46) (8 rows x 128 B) | layout SWIZZLE_128B=1 [62,64).  Tiles are 1024-byte aligned (base offset 0).
 __device__ __forceinline__ uint64_t make_desc(const void *smem) {
   uint64_t d = (uint64_t)((smem_u32(smem) & 0x3ffff) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, N=BN, M=BM
-__device__ __forceinline__ uint32_t make_idesc() {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t *r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, bf16 in, fp32 accumulate; scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_bf16(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
 // logistic_func, calc_dnn.c:362-369
@@ -100,268 +89,109 @@ struct GemmArgs {
 };
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-dnn_gemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-                const GemmArgs g) {
+dnn_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
+               const GemmArgs g) {
   extern __shared__ unsigned char dsm_raw[];
   unsigned char *dsm = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(dsm_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full = reinterpret_cast<uint64_t *>(dsm + STAGES * STAGE_BYTES);
   uint64_t *empty = full + STAGES;
-  uint64_t *tmem_full = empty + STAGES;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_full + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = (g.K + BK - 1) / BK;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    mbar_fence_init();
-  }
-  if (warp == 2) {   // TMEM: 128 fp32 columns for the 128x128 accumulator
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(128u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer =====
-      for (int kb = 0; kb < nkb; kb++) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        unsigned char *st = dsm + s * STAGE_BYTES;
-        mbar_expect_tx(&full[s], STAGE_BYTES);
-        tma_load_2d(st, &map_a_hi, &full[s], kb * BK, m0);
-        tma_load_2d(st + TILE_BYTES, &map_a_lo, &full[s], kb * BK, m0);
-        tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, &full[s], kb * BK, n0);
-        tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, &full[s], kb * BK, n0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer: three bf16 products per k-step into one fp32 accumulator =====
-      const uint32_t idesc = make_idesc();
-      for (int kb = 0; kb < nkb; kb++) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        unsigned char *st = dsm + s * STAGE_BYTES;
-        const uint64_t a_hi = make_desc(st), a_lo = make_desc(st + TILE_BYTES);
-        const uint64_t b_hi = make_desc(st + 2 * TILE_BYTES), b_lo = make_desc(st + 3 * TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < BK / 16; k++) {
-          const uint64_t adv = (uint64_t)(k * 32 >> 4);      // 16 bf16 = 32 bytes along K inside the swizzle atom
-          tc_mma_bf16(tmem_base, a_hi + adv, b_hi + adv, idesc, (kb | k) ? 1u : 0u);
-          tc_mma_bf16(tmem_base, a_hi + adv, b_lo + adv, idesc, 1u);
-          tc_mma_bf16(tmem_base, a_lo + adv, b_hi + adv, idesc, 1u);
-        }
-        tc_commit(&empty[s]);                                  // frees the stage when these MMAs retire
-      }
-      tc_commit(tmem_full);                                    // accumulator complete
-    }
-  } else {
-    // ===== epilogue: TMEM -> registers -> bias / logistic / split -> global =====
-    const int q = warp & 3;                                    // TMEM lane quarter this warp may access
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int row = m0 + q * 32 + lane;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; c++) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-      const int col0 = n0 + c * 32;
-      if (row < g.M) {
-        if (g.last) {
-          float *dst = g.logits + (size_t)row * g.ld_logits + col0;
-#pragma unroll
-          for (int i = 0; i < 32; i++)
-            if (col0 + i < g.N) dst[i] = __uint_as_float(r[i]) + __ldg(g.bias + col0 + i);
-        } else {
-          __align__(16) __nv_bfloat16 hi[32], lo[32];
-#pragma unroll
-          for (int i = 0; i < 32; i++) {
-            float v = 0.0f;
-            if (col0 + i < g.N) v = logistic_ref(__uint_as_float(r[i]) + __ldg(g.bias + col0 + i), g.logistic);
-            const __nv_bfloat16 h = __float2bfloat16_rn(v);
-            hi[i] = h;
-            lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-          }
-          // ld_out is a multiple of 8 and col0 of 32: 16-byte aligned vector stores; columns beyond N
-          // (up to ld_out) are written as zeros so the next layer's K tail is clean
-          uint4 *dh = reinterpret_cast<uint4 *>(g.out_hi + (size_t)row * g.ld_out + col0);
-          uint4 *dl = reinterpret_cast<uint4 *>(g.out_lo + (size_t)row * g.ld_out + col0);
-#pragma unroll
-          for (int v4 = 0; v4 < 4; v4++)
-            if (col0 + v4 * 8 < g.ld_out) { dh[v4] = reinterpret_cast<const uint4 *>(hi)[v4]; dl[v4] = reinterpret_cast<const uint4 *>(lo)[v4]; }
-        }
-      }
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(128u) : "memory");
-  }
-}
-
-// ---- persistent variant -----------------------------------------------------------------------------
-// One CTA per SM walks the output tiles (column blocks fastest, so the CTAs that run side by side share the
-// activation rows in L2); the accumulator is double-buffered in TMEM, so the four epilogue warps drain tile i
-// (tcgen05.ld, bias, table logistic, bf16 hi/lo split, stores) while the MMA warp is already filling tile i+1
-// and the TMA warp runs ahead through the shared-memory ring.  BN_ = 128 (3 stages of 64 KB) or 256 (2 stages of
-// 96 KB: a 128x256 tile moves 1.5x the bytes for 2x the flops -- the kernel is bound by the L2 -> shared-memory
-// path, see DESIGN.md K2).
-template <int BN_>
-struct PersistentCfg {
-  static constexpr int STAGES_ = (BN_ == 128) ? 3 : 2;
-  static constexpr int B_TILE = BN_ * BK * 2;
-  static constexpr int STAGE = 2 * TILE_BYTES + 2 * B_TILE;     // A_hi A_lo B_hi B_lo
-  static constexpr int SMEM = STAGES_ * STAGE + 1024 + 256;
-};
-
-template <int BN_>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-dnn_gemm_persistent(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                    const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-                    const GemmArgs g) {
-  using Cfg = PersistentCfg<BN_>;
-  constexpr int S = Cfg::STAGES_;
-  extern __shared__ unsigned char dsm_raw[];
-  unsigned char *dsm = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(dsm_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full = reinterpret_cast<uint64_t *>(dsm + S * Cfg::STAGE);
-  uint64_t *empty = full + S;
-  uint64_t *tmem_full = empty + S;          // [2]
-  uint64_t *tmem_empty = tmem_full + 2;     // [2]
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkb = (g.K + BK - 1) / BK;
-  const int n_nblk = (g.N + BN_ - 1) / BN_, n_mblk = (g.M + BM - 1) / BM;
+  const int n_nblk = (g.N + BN - 1) / BN, n_mblk = (g.M + BM - 1) / BM;
   const int n_tiles = n_nblk * n_mblk;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 4); }
+    for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMERS * 4); }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN_)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
       int it = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int m0 = (tile / n_nblk) * BM, n0 = (tile % n_nblk) * BN_;
+        const int m0 = (tile / n_nblk) * BM, n0 = (tile % n_nblk) * BN;
         for (int kb = 0; kb < nkb; kb++, it++) {
-          const int s = it % S;
-          const uint32_t ph = (it / S) & 1;
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
           mbar_wait(&empty[s], ph ^ 1);
-          unsigned char *st = dsm + s * Cfg::STAGE;
-          mbar_expect_tx(&full[s], Cfg::STAGE);
+          unsigned char *st = dsm + s * STAGE_BYTES;
+          mbar_expect_tx(&full[s], STAGE_BYTES);
           tma_load_2d(st, &map_a_hi, &full[s], kb * BK, m0);
           tma_load_2d(st + TILE_BYTES, &map_a_lo, &full[s], kb * BK, m0);
-          unsigned char *bh = st + 2 * TILE_BYTES, *bl = bh + Cfg::B_TILE;
-#pragma unroll
-          for (int h = 0; h < BN_ / 128; h++) {                 // the weight maps have 128-row boxes
-            tma_load_2d(bh + h * TILE_BYTES, &map_b_hi, &full[s], kb * BK, n0 + h * 128);
-            tma_load_2d(bl + h * TILE_BYTES, &map_b_lo, &full[s], kb * BK, n0 + h * 128);
-          }
+          tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, &full[s], kb * BK, n0);
+          tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, &full[s], kb * BK, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN_ >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int it = 0, i = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, i++) {
-        const int b = i & 1;
-        mbar_wait(&tmem_empty[b], (uint32_t)((i >> 1) & 1) ^ 1u);    // the epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(b * BN_);
-        for (int kb = 0; kb < nkb; kb++, it++) {
-          const int s = it % S;
-          const uint32_t ph = (it / S) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          unsigned char *st = dsm + s * Cfg::STAGE;
-          const uint64_t a_hi = make_desc(st), a_lo = make_desc(st + TILE_BYTES);
-          const uint64_t b_hi = make_desc(st + 2 * TILE_BYTES), b_lo = make_desc(st + 2 * TILE_BYTES + Cfg::B_TILE);
-#pragma unroll
-          for (int k = 0; k < BK / 16; k++) {
-            const uint64_t adv = (uint64_t)(k * 32 >> 4);
-            tc_mma_bf16(acc, a_hi + adv, b_hi + adv, idesc, (kb | k) ? 1u : 0u);
-            tc_mma_bf16(acc, a_hi + adv, b_lo + adv, idesc, 1u);
-            tc_mma_bf16(acc, a_lo + adv, b_hi + adv, idesc, 1u);
-          }
-          tc_commit(&empty[s]);
-        }
-        tc_commit(&tmem_full[b]);
-      }
-    }
-  } else {
-    // ===== epilogue warps =====
-    const int q = warp & 3;
-    int i = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, i++) {
-      const int b = i & 1;
-      const int m0 = (tile / n_nblk) * BM, n0 = (tile % n_nblk) * BN_;
-      mbar_wait(&tmem_full[b], (uint32_t)((i >> 1) & 1));
-      tc_fence_after();
-      const int row = m0 + q * 32 + lane;
-#pragma unroll 1
-      for (int c = 0; c < BN_ / 32; c++) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * BN_ + c * 32), r);
-        const int col0 = n0 + c * 32;
-        if (row < g.M) {
-          if (g.last) {
-            float *dst = g.logits + (size_t)row * g.ld_logits + col0;
-#pragma unroll
-            for (int e = 0; e < 32; e++)
-              if (col0 + e < g.N) dst[e] = __uint_as_float(r[e]) + __ldg(g.bias + col0 + e);
-          } else {
-            __align__(16) __nv_bfloat16 hi[32], lo[32];
-#pragma unroll
-            for (int e = 0; e < 32; e++) {
-              float v = 0.0f;
-              if (col0 + e < g.N) v = logistic_ref(__uint_as_float(r[e]) + __ldg(g.bias + col0 + e), g.logistic);
-              const __nv_bfloat16 h = __float2bfloat16_rn(v);
-              hi[e] = h;
-              lo[e] = __float2bfloat16_rn(v - __bfloat162float(h));
-            }
-            uint4 *dh = reinterpret_cast<uint4 *>(g.out_hi + (size_t)row * g.ld_out + col0);
-            uint4 *dl = reinterpret_cast<uint4 *>(g.out_lo + (size_t)row * g.ld_out + col0);
-#pragma unroll
-            for (int v4 = 0; v4 < 4; v4++)
-              if (col0 + v4 * 8 < g.ld_out) { dh[v4] = reinterpret_cast<const uint4 *>(hi)[v4]; dl[v4] = reinterpret_cast<const uint4 *>(lo)[v4]; }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[b]);               // 4 arrivals (one per epilogue warp) free the accumulator
-    }
+    return;
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"((uint32_t)(2 * BN_)) : "memory");
+
+  // ===== consumer warpgroups: rows [64*c, 64*c+64) of every tile =====
+  const int c = wg - 1;
+  const int wl = warp & 3;                                     // warp inside the warpgroup
+  float d[64];
+  int it = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int m0 = (tile / n_nblk) * BM, n0 = (tile % n_nblk) * BN;
+    for (int kb = 0; kb < nkb; kb++, it++) {
+      const int s = it % STAGES;
+      mbar_wait(&full[s], (it / STAGES) & 1);
+      unsigned char *st = dsm + s * STAGE_BYTES;
+      const uint64_t a_hi = make_desc(st + c * (64 * 128)), a_lo = make_desc(st + TILE_BYTES + c * (64 * 128));
+      const uint64_t b_hi = make_desc(st + 2 * TILE_BYTES), b_lo = make_desc(st + 3 * TILE_BYTES);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; k++) {
+        const uint64_t adv = (uint64_t)(k * 32 >> 4);        // 16 bf16 = 32 bytes along K inside the swizzle atom
+        wgmma_bf16(d, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
+        wgmma_bf16(d, a_hi + adv, b_lo + adv, 1u);
+        wgmma_bf16(d, a_lo + adv, b_hi + adv, 1u);
+      }
+      wg_commit();
+      // the previous k-block's group has retired once at most this one is pending: hand its stage back
+      wg_wait<1>();
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+      }
+    }
+    wg_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+
+    // ===== epilogue from registers: element (row, col) of d[4j + 2h + e] is
+    //       row = 16*wl + lane/4 + 8h, col = 8j + 2*(lane%4) + e =====
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int row = m0 + c * 64 + wl * 16 + (lane >> 2) + 8 * h;
+      if (row >= g.M) continue;
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        const int col = n0 + 8 * j + 2 * (lane & 3);
+        const float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
+        if (g.last) {
+          float *dst = g.logits + (size_t)row * g.ld_logits + col;
+          if (col < g.N) dst[0] = x0 + __ldg(g.bias + col);
+          if (col + 1 < g.N) dst[1] = x1 + __ldg(g.bias + col + 1);
+        } else if (col < g.ld_out) {
+          // ld_out is a multiple of 8 and col even: col + 1 < ld_out too.  Columns beyond N (up to ld_out) are
+          // written as zeros so the next layer's K tail is clean
+          const float v0 = (col < g.N) ? logistic_ref(x0 + __ldg(g.bias + col), g.logistic) : 0.0f;
+          const float v1 = (col + 1 < g.N) ? logistic_ref(x1 + __ldg(g.bias + col + 1), g.logistic) : 0.0f;
+          const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
+          __nv_bfloat162 hi, lo;
+          hi.x = h0; hi.y = h1;
+          lo.x = __float2bfloat16_rn(v0 - __bfloat162float(h0));
+          lo.y = __float2bfloat16_rn(v1 - __bfloat162float(h1));
+          *reinterpret_cast<__nv_bfloat162 *>(g.out_hi + (size_t)row * g.ld_out + col) = hi;
+          *reinterpret_cast<__nv_bfloat162 *>(g.out_lo + (size_t)row * g.ld_out + col) = lo;
+        }
+      }
+    }
   }
 }
 
@@ -420,13 +250,6 @@ dnn_softmax_kernel(const float *__restrict__ logits, int ld_logits, int N, const
 
 }  // namespace jb200
 
-namespace jb200 {
-// dnn_cluster.cu (experimental, JB200_DNN_KERNEL=2)
-int dnn_launch_cluster2(const CUtensorMap &ma_hi, const CUtensorMap &ma_lo, const CUtensorMap &mw_hi, const CUtensorMap &mw_lo,
-                        int M, int N, int K, const float *bias, const float *logistic, __nv_bfloat16 *out_hi, __nv_bfloat16 *out_lo,
-                        int ld_out, float *logits, int ld_logits, int last, int n_sm, cudaStream_t st);
-}
-
 // =============================================================================================
 using namespace jb200;
 
@@ -448,7 +271,7 @@ struct jb200_dnn {
   PFN_encodeTiled encode = nullptr;
   cudaStream_t stream = nullptr;
   // batch buffers
-  int cap_frames = 0, max_width = 0, ld_logits = 0, n_sm = 0, variant = 256;
+  int cap_frames = 0, max_width = 0, ld_logits = 0, n_sm = 0;
   float *d_in = nullptr, *d_logits = nullptr, *d_rows = nullptr;
   __nv_bfloat16 *act_hi[2] = {nullptr, nullptr}, *act_lo[2] = {nullptr, nullptr};
 };
@@ -483,7 +306,7 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
   JB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   JB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) { set_error("device is sm_%d%d; tcgen05 needs sm_100a", prop.major, prop.minor); return JB200_ERR_NODEVICE; }
+  if (prop.major != 9) { set_error("device is sm_%d%d; the wgmma GEMM needs sm_90a", prop.major, prop.minor); return JB200_ERR_NODEVICE; }
   jb200_dnn *h = new jb200_dnn();
   h->device = device; h->n_layers = d->n_layers; h->in_dim = d->in_dim; h->out_dim = d->out_dim;
   h->row_stride = (d->out_dim + 3) & ~3;
@@ -527,11 +350,8 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
     JB_CUDA(cudaMemcpy(h->d_logistic, tbl.data(), sizeof(float) * LOGISTIC_N, cudaMemcpyHostToDevice));
   }
   h->ld_logits = (d->out_dim + 3) & ~3;
-  JB_CUDA(cudaFuncSetAttribute(dnn_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  JB_CUDA(cudaFuncSetAttribute(dnn_gemm_persistent<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PersistentCfg<128>::SMEM));
-  JB_CUDA(cudaFuncSetAttribute(dnn_gemm_persistent<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, PersistentCfg<256>::SMEM));
+  JB_CUDA(cudaFuncSetAttribute(dnn_gemm_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   h->n_sm = prop.multiProcessorCount;
-  h->variant = getenv("JB200_DNN_KERNEL") ? atoi(getenv("JB200_DNN_KERNEL")) : 256;   // 0 one tile per CTA, 128 / 256 persistent, 2 = experimental 2-CTA cluster (dnn_cluster.cu)
   *out = h;
   return JB200_OK;
 }
@@ -579,22 +399,8 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
     g.out_hi = h->act_hi[cur ^ 1]; g.out_lo = h->act_lo[cur ^ 1];
     g.ld_out = g.last ? 0 : h->L[l + 1].ld_in;
     g.logits = h->d_logits; g.ld_logits = h->ld_logits;
-    if (h->variant == 0) {
-      dim3 grid((L.out + BN - 1) / BN, (T + BM - 1) / BM);
-      dnn_gemm_kernel<<<grid, GEMM_THREADS, GEMM_SMEM, st>>>(ma_hi, ma_lo, L.map_w_hi, L.map_w_lo, g);
-    } else if (h->variant == 128) {
-      const int tiles = ((L.out + 127) / 128) * ((T + BM - 1) / BM);
-      dnn_gemm_persistent<128><<<std::min(tiles, h->n_sm), GEMM_THREADS, PersistentCfg<128>::SMEM, st>>>(ma_hi, ma_lo, L.map_w_hi, L.map_w_lo, g);
-    } else if (h->variant == 2) {
-      rc = dnn_launch_cluster2(ma_hi, ma_lo, L.map_w_hi, L.map_w_lo, g.M, g.N, g.K, g.bias, g.logistic, g.out_hi, g.out_lo,
-                               g.ld_out, g.logits, g.ld_logits, g.last, h->n_sm, st);
-      if (rc) return rc;
-      cur ^= 1;
-      continue;
-    } else {
-      const int tiles = ((L.out + 255) / 256) * ((T + BM - 1) / BM);
-      dnn_gemm_persistent<256><<<std::min(tiles, h->n_sm), GEMM_THREADS, PersistentCfg<256>::SMEM, st>>>(ma_hi, ma_lo, L.map_w_hi, L.map_w_lo, g);
-    }
+    const int tiles = ((L.out + BN - 1) / BN) * ((T + BM - 1) / BM);
+    dnn_gemm_wgmma<<<std::min(tiles, h->n_sm), GEMM_THREADS, GEMM_SMEM, st>>>(ma_hi, ma_lo, L.map_w_hi, L.map_w_lo, g);
     JB_LAUNCH_CHECK();
     cur ^= 1;
   }

@@ -7,7 +7,7 @@
 // and for outprob_cd (outprob.c:286-400) in the cd-set kernel.
 //
 // Layout in HBM.  One 16-byte aligned record per Gaussian, in quads so that a 64-bit register pair
-// holds two dimensions for the packed fp32x2 FMA (FFMA2):
+// holds two dimensions (a dimension pair is carried through the inner loop as one 64-bit value):
 //      [ (m0 m1 iv0 iv1) (m2 m3 iv2 iv3) ... (m38 gconst iv38 lnw) ]   (2D+2 floats -> 320 B for D=39)
 // Records of a state are contiguous and states follow each other, so a tile of states is ONE
 // contiguous byte range that a single 1-D bulk (TMA) copy stages into shared memory
@@ -43,18 +43,16 @@ __host__ __device__ constexpr int rec_ivar(int d) { return 4 * (d >> 1) + 2 + (d
 __host__ __device__ constexpr int rec_gconst(int D) { return (D & 1) ? 4 * (D >> 1) + 1 : 2 * D; }
 __host__ __device__ constexpr int rec_lnw(int D) { return (D & 1) ? 4 * (D >> 1) + 3 : 2 * D + 1; }
 
-// packed fp32x2 FMA (SASS FFMA2): one issue slot for two lanes' worth of work.  Every use below is an
-// exactly-rounded single operation (a*b+0, a*(-1)+c), so the exact mode stays bit-identical.
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
   return ((unsigned long long)__float_as_uint(hi) << 32) | __float_as_uint(lo);
 }
 __device__ __forceinline__ float lo2(unsigned long long v) { return __uint_as_float((unsigned)(v & 0xffffffffu)); }
 __device__ __forceinline__ float hi2(unsigned long long v) { return __uint_as_float((unsigned)(v >> 32)); }
+// FMA on a dimension pair: two scalar FFMAs (sm_90 has no packed fp32x2 FMA).  Every use below is an
+// exactly-rounded single operation (a*b+0, a*(-1)+c), so the exact mode stays bit-identical.
+__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
+  return pack2(__fmaf_rn(lo2(a), lo2(b), lo2(c)), __fmaf_rn(hi2(a), hi2(b), hi2(c)));
+}
 
 __device__ __forceinline__ float addlog_step_exact(float y, float x, const float *__restrict__ tbl) {
   // addlog.c:112-120
@@ -120,7 +118,7 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
 
   // this thread's frames, in registers
   float v[GMM_FPT][D];                       // scalar copy (pruned variant)
-  unsigned long long v2[GMM_FPT][NQ];        // the same, packed (x_2q, x_2q+1) for the FFMA2 path
+  unsigned long long v2[GMM_FPT][NQ];        // the same, paired (x_2q, x_2q+1) for the fma2 path
   // T counts LOGICAL frames.  With a segment list (the batch pipeline scores one time slice of every utterance per
   // launch) logical frame f is frame seg_start[s] + f - seg_off[s] of the feature / score matrices, s = its segment
   int fr[GMM_FPT];
@@ -341,7 +339,7 @@ struct jb200_gmm {
   cudaStream_t stream = nullptr;
   // scratch for the host variants
   float *d_feats = nullptr, *d_rows = nullptr; size_t cap_frames = 0;
-  int sm_count = 148;
+  int sm_count = 132;
 };
 
 namespace jb200 {
@@ -375,7 +373,7 @@ extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, j
   JB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   JB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) { set_error("device %d is sm_%d%d; libjb200 is built for sm_100a only", device, prop.major, prop.minor); return JB200_ERR_NODEVICE; }
+  if (prop.major != 9) { set_error("device %d is sm_%d%d; libjb200 is built for sm_90a only", device, prop.major, prop.minor); return JB200_ERR_NODEVICE; }
 
   jb200_gmm *h = new jb200_gmm();
   h->device = device; h->mode = mode; h->sm_count = prop.multiProcessorCount;

@@ -24,7 +24,7 @@
 #include <julius/juliuslib.h>
 #include "jb200_model.h"
 
-#define PLUGIN_TITLE "jb200 model flattener (B200 acoustic scoring + pass-1 beam)"
+#define PLUGIN_TITLE "jb200 model flattener (GPU acoustic scoring + pass-1 beam)"
 
 /* ---------------------------------------------------------------- tiny pointer map */
 typedef struct { const void **k; int *v; int cap, n; } PMap;

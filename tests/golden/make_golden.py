@@ -8,6 +8,10 @@ Each fixture directory holds
     out.jrf     reference outputs: [T x S] state scores, word trellis, pass-1 best
     feats.npz   the input feature matrices (u0, u1, ...)
     meta.json   the jconf-style options used
+
+    python tests/golden/make_golden.py sweep
+
+writes the option sweeps of tests/test_oracle_sweep.py as sweep/<case>.npz, in a compact form (tests/util.py).
 """
 import json
 import os
@@ -19,8 +23,10 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-from julius_b200 import synth  # noqa: E402
+from julius_b200 import refdump, synth  # noqa: E402
 from oracle import ffi, fixtures  # noqa: E402
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import util  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -45,6 +51,8 @@ CASES = {
     # user-defined LM functions on top of the N-gram (-userlm, wchmm.h:274-276; registered by the driver, JREF_USERLM=1)
     "small_userlm": ("small", 2, 200, 1, ["-userlm", "-b", "100"]),
 }
+# cases whose model.jb2m would exceed 1 MB: stored as a compressed delta against the model of another case (tests/util.py)
+COMPACT = {"small_userlm": "small_b100", "small_tm": None}
 # cases that need something in the driver's environment
 CASE_ENV = {"small_userlm": {"JREF_USERLM": "1"}}
 # DNN-HMM: (preset, DnnConfig kwargs, n_utts, n_frames, extra args)
@@ -56,8 +64,24 @@ DNN_CASES = {
 }
 
 
+def make_sweep():
+    from test_oracle_sweep import SWEEP, GRAMMAR_SWEEP
+    cases = [(p, e, False, dict(n_utts=2, n_frames=150, noise_utts=1)) for p, e in SWEEP]
+    cases += [("small", e, True, dict(n_utts=2, n_frames=180, noise_utts=1)) for e in GRAMMAR_SWEEP]
+    for preset, extra, grammar, kw in cases:
+        tmp = tempfile.mkdtemp(prefix="jb200_golden_")
+        m, files, dump, out = fixtures.make_fixture(preset, tmp, extra_args=extra, grammar=grammar, **kw)
+        blob = refdump.load_blob(os.path.join(tmp, "model.jb2m"))
+        feats = [synth.read_htk_param(fn)[0] for fn in files]
+        dst = util.write_sweep_case(preset, extra, grammar, blob, feats, refdump.load_refdump(dump))
+        shutil.rmtree(tmp)
+        print(" ".join([preset] + extra), "->", dst)
+
+
 def main():
     ffi.build()
+    if sys.argv[1:] == ["sweep"]:
+        return make_sweep()
     only = set(sys.argv[1:])
     for name, (preset, nu, nf, nn, extra) in CASES.items():
         if only and name not in only:
@@ -67,13 +91,17 @@ def main():
                                                     grammar=name in GRAMMAR_CASES, env_extra=CASE_ENV.get(name))
         dst = os.path.join(HERE, name)
         os.makedirs(dst, exist_ok=True)
-        shutil.copy(os.path.join(tmp, "model.jb2m"), dst)
+        meta = {"preset": preset, "extra_args": extra, "n_utts": len(files), "grammar": name in GRAMMAR_CASES, "env": CASE_ENV.get(name, {}),
+                "summary": out.strip().splitlines()[-1]}
+        if name in COMPACT:
+            util.write_golden_model(dst, refdump.load_blob(os.path.join(tmp, "model.jb2m")), COMPACT[name], meta)
+        else:
+            shutil.copy(os.path.join(tmp, "model.jb2m"), dst)
         shutil.copy(dump, os.path.join(dst, "out.jrf"))
         feats = {f"u{i}": synth.read_htk_param(fn)[0] for i, fn in enumerate(files)}
         np.savez_compressed(os.path.join(dst, "feats.npz"), **feats)
         with open(os.path.join(dst, "meta.json"), "w") as f:
-            json.dump({"preset": preset, "extra_args": extra, "n_utts": len(files), "grammar": name in GRAMMAR_CASES, "env": CASE_ENV.get(name, {}),
-                       "summary": out.strip().splitlines()[-1]}, f, indent=1)
+            json.dump(meta, f, indent=1)
         shutil.rmtree(tmp)
         print(name, "->", dst)
     for name, (preset, dkw, nu, nf, extra) in DNN_CASES.items():

@@ -1,4 +1,4 @@
-"""GPU: K2 DNN-HMM forward (tcgen05 bf16x3 GEMM stack) through the C-ABI vs the reference's golden scores."""
+"""GPU: K2 DNN-HMM forward (wgmma bf16x3 GEMM stack) through the C-ABI vs the reference's golden scores."""
 import numpy as np
 import pytest
 
@@ -59,10 +59,13 @@ def full_dnn():
     return desc.Descriptors(full_dnn_blob())
 
 
-@pytest.mark.parametrize("T", [1, 127, 129, 300])
+@pytest.mark.parametrize("T", [1, 127, 129, 300, 1100, 2200])
 def test_dnn_full_shape_within_1e4_of_the_oracle(full_dnn, T, oracle_lib):
-    """K2 at the BASELINE configs[3] shape, 528 -> 7 x 2048 -> 3000: 24 k-blocks per hidden layer, a partial last
-    column block (3000 = 11 x 256 + 184), TMEM double-buffer wrap-around, ragged frame counts around the 128-row tile.
+    """K2 at the BASELINE configs[3] shape, 528 -> 7 x 2048 -> 3000: 32 k-blocks per hidden layer, a partial last
+    column block (3000 = 23 x 128 + 56), ragged frame counts around the 128-row tile.  The GEMM runs one persistent CTA per
+    SM at most: T = 1100 gives 9 x 16 hidden-layer and 9 x 24 last-layer tiles, T = 2200 18 x 16 and 18 x 24, more than the
+    132 SMs of an H100 in both, so CTAs take a second (and third) tile -- the operand ring carried across tiles, the next
+    tile's loads issued during an epilogue, the accumulator restarted at each tile's first k-step.
     The checker is the CPU restatement of dnn_calc_outprob (calc_dnn.c:774-868), itself pinned bit-exact to the
     compiled reference on the golden DNN cases."""
     x = synth.sample_dnn_input(np.random.default_rng(100 + T), T, 528)

@@ -1,19 +1,16 @@
 """GPU: the CUDA path against the compiled reference across jconf options beyond the committed golden cases --
-the device-side twin of tests/test_oracle_sweep.py.  Each case samples fresh utterances, pushes them through the
-compiled reference (oracle/_ref/jref, which travels with the tree) and through K1 + K3, and demands bit-identical
-state scores and an identical word trellis.  Covers -iwcd1 avg / best N, -lmp, score-envelope pruning (-bs),
--gprune heuristic, -iwsp, transparent words, flattened tied-mixture codebooks and DFA grammars on the device."""
-import os
-
+the device-side twin of tests/test_oracle_sweep.py.  Each case's utterances (decoded by the compiled reference, stored
+under tests/golden/sweep/) go through K1 + K3, which must reproduce the reference's state scores bit for bit and its
+word trellis exactly.  Covers -iwcd1 avg / best N, -lmp, score-envelope pruning (-bs), -gprune heuristic, -iwsp,
+transparent words, flattened tied-mixture codebooks and DFA grammars on the device."""
 import numpy as np
 import pytest
 
-from julius_b200 import capi, desc, refdump, synth
-from util import ROOT, atoms_equal
+from julius_b200 import capi
+from util import atoms_equal, load_sweep_case, scores_sha
 from test_oracle_sweep import SWEEP, GRAMMAR_SWEEP
 
 pytestmark = pytest.mark.gpu
-JREF = os.path.join(ROOT, "oracle", "_ref", "jref")
 
 
 def _check(r, u):
@@ -23,34 +20,21 @@ def _check(r, u):
     assert np.float32(r["score"]) == np.float32(u.score)
 
 
-@pytest.mark.skipif(not os.path.exists(JREF), reason="compiled reference (oracle/_ref/jref) not present")
 @pytest.mark.parametrize("preset,extra", SWEEP, ids=[" ".join([p] + e) for p, e in SWEEP])
-def test_gpu_path_equals_compiled_reference(preset, extra, tmp_path):
-    from oracle import fixtures
-    d = str(tmp_path)
-    m, files, dump, out = fixtures.make_fixture(preset, d, n_utts=2, n_frames=150, extra_args=extra, noise_utts=1)
-    ds = desc.Descriptors(refdump.load_blob(os.path.join(d, "model.jb2m")))
-    utts = refdump.load_refdump(dump)
-    feats = [synth.read_htk_param(fn)[0] for fn in files]
+def test_gpu_path_equals_compiled_reference(preset, extra):
+    ds, feats, utts = load_sweep_case(preset, extra)
     am = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
     for u, x in zip(utts, feats):
-        sc = am.score(x)
-        assert np.array_equal(sc.view(np.uint32), u.outprob.view(np.uint32)), "state scores differ from the reference"
+        assert scores_sha(am.score(x)) == u.outprob_sha256, "state scores differ from the reference"
     dec = capi.Decoder(ds, am, max_utts=4, max_frames=2048)
     for r, u in zip(dec.decode(feats), utts):
         _check(r, u)
 
 
 # the GPU beam takes grammars on normal trees only (creation refuses -multipath loudly, tested in test_gpu_beam.py)
-@pytest.mark.skipif(not os.path.exists(JREF), reason="compiled reference (oracle/_ref/jref) not present")
 @pytest.mark.parametrize("extra", [e for e in GRAMMAR_SWEEP if "-multipath" not in e], ids=lambda e: " ".join(e))
-def test_gpu_grammar_mode_equals_compiled_reference(extra, tmp_path):
-    from oracle import fixtures
-    d = str(tmp_path)
-    m, files, dump, out = fixtures.make_fixture("small", d, n_utts=2, n_frames=180, extra_args=extra, noise_utts=1, grammar=True)
-    ds = desc.Descriptors(refdump.load_blob(os.path.join(d, "model.jb2m")))
-    utts = refdump.load_refdump(dump)
-    feats = [synth.read_htk_param(fn)[0] for fn in files]
+def test_gpu_grammar_mode_equals_compiled_reference(extra):
+    ds, feats, utts = load_sweep_case("small", extra, grammar=True)
     am = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
     dec = capi.Decoder(ds, am, max_utts=4, max_frames=2048)
     for r, u in zip(dec.decode(feats), utts):

@@ -86,7 +86,7 @@ def test_descriptor_layouts_match_the_c_header(tmp_path):
 
 
 def test_product_path_fails_loudly_without_a_device():
-    """No CPU fallback: on a machine without an sm_100 GPU every create call of the C-ABI must return an error (and the
+    """No CPU fallback: on a machine without an sm_90 GPU every create call of the C-ABI must return an error (and the
     Python mirror raise), never hand back a handle that computes on the host."""
     import torch
     if torch.cuda.is_available():

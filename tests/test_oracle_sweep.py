@@ -1,14 +1,12 @@
-"""CPU: the restatement against the compiled reference itself (oracle/_ref/jref), across jconf options beyond the
-committed golden cases.  Runs wherever the compiled reference is present (it is built from /root/reference by
-oracle/Makefile and travels with the tree); each case pushes freshly sampled utterances through the reference and
-through the restatement and demands bit-identical state scores and an identical word trellis."""
+"""CPU: the restatement against the compiled reference itself, across jconf options beyond the committed golden
+cases.  Each case's utterances were decoded by the compiled reference (tests/golden/make_golden.py sweep, stored under
+tests/golden/sweep/); the restatement must reproduce its state scores bit for bit and its word trellis exactly."""
 import os
 
 import numpy as np
 import pytest
 
-from julius_b200 import desc, refdump, synth
-from util import ROOT, atoms_equal
+from util import ROOT, atoms_equal, load_sweep_case, scores_sha
 
 JREF = os.path.join(ROOT, "oracle", "_ref", "jref")
 
@@ -29,18 +27,16 @@ SWEEP = [
 GRAMMAR_SWEEP = [["-b", "100"], ["-b", "60", "-penalty1", "-2.5", "-iwcd1", "max"], ["-b", "150", "-multipath", "-penalty1", "1.5"]]
 
 
-@pytest.mark.skipif(not os.path.exists(JREF), reason="compiled reference (oracle/_ref/jref) not present")
 @pytest.mark.parametrize("extra", GRAMMAR_SWEEP, ids=[" ".join(e) for e in GRAMMAR_SWEEP])
-def test_grammar_mode_restatement_equals_compiled_reference(extra, tmp_path, oracle_lib):
+def test_grammar_mode_restatement_equals_compiled_reference(extra, oracle_lib):
     """Grammar (DFA) recognition: category tree, category-pair constraint, insertion penalty, all sentence-initial
     words alive at frame 0, best atom of the last frame as the pass-1 result (beam.c:1669-1760, :2404-2455, :435-458)."""
-    from oracle import fixtures
-    d = str(tmp_path)
-    m, files, dump, out = fixtures.make_fixture("small", d, n_utts=2, n_frames=180, extra_args=extra, noise_utts=1, grammar=True)
-    ds = desc.Descriptors(refdump.load_blob(os.path.join(d, "model.jb2m")))
+    ds, feats, utts = load_sweep_case("small", extra, grammar=True)
     assert ds.tree.lm_type == 1 and ds.tree.n_shared == 0 and ds.tree.n_init >= 1
-    for u in refdump.load_refdump(dump):
-        r = oracle_lib.beam_decode(ds, u.outprob)
+    for x, u in zip(feats, utts):
+        sc = oracle_lib.gmm_score(ds, x)
+        assert scores_sha(sc) == u.outprob_sha256, "state scores differ from the reference"
+        r = oracle_lib.beam_decode(ds, sc)
         ok, why = atoms_equal(r["atoms"], u.atoms)
         assert ok, why
         assert r["words"] == u.words and r["status"] == u.status
@@ -56,20 +52,13 @@ def test_tied_mixture_with_history_dependent_pruning_is_refused(tmp_path):
         fixtures.make_fixture("small_tm", str(tmp_path), n_utts=1, n_frames=50, extra_args=["-b", "60"])
 
 
-@pytest.mark.skipif(not os.path.exists(JREF), reason="compiled reference (oracle/_ref/jref) not present")
 @pytest.mark.parametrize("preset,extra", SWEEP, ids=[" ".join([p] + e) for p, e in SWEEP])
-def test_restatement_equals_compiled_reference(preset, extra, tmp_path, oracle_lib):
-    from oracle import fixtures
-    d = str(tmp_path)
-    m, files, dump, out = fixtures.make_fixture(preset, d, n_utts=1, n_frames=150, extra_args=extra, noise_utts=1)
-    ds = desc.Descriptors(refdump.load_blob(os.path.join(d, "model.jb2m")))
-    utts = refdump.load_refdump(dump)
-    assert len(utts) == len(files)
-    for u, fn in zip(utts, files):
-        x, _ = synth.read_htk_param(fn)
+def test_restatement_equals_compiled_reference(preset, extra, oracle_lib):
+    ds, feats, utts = load_sweep_case(preset, extra)
+    for u, x in zip(utts, feats):
         sc = oracle_lib.gmm_score(ds, x)
-        assert np.array_equal(sc.view(np.uint32), u.outprob.view(np.uint32))
-        r = oracle_lib.beam_decode(ds, u.outprob)
+        assert scores_sha(sc) == u.outprob_sha256, "state scores differ from the reference"
+        r = oracle_lib.beam_decode(ds, sc)
         ok, why = atoms_equal(r["atoms"], u.atoms)
         assert ok, why
         assert r["words"] == u.words and r["status"] == u.status

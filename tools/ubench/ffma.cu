@@ -1,7 +1,7 @@
 // ffma.cu -- FP32 SIMT peak of the device as a kernel can reach it: 8 independent FFMA chains per thread, 1024 threads
-// per SM x 4 resident blocks, no memory traffic.  Denominator of roofline_scoring for the GMM kernel (bench.py reads
-// profiles/fp32_peak.json, which a run of this program prints).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ffma ffma.cu
+// per SM x 4 resident blocks, no memory traffic: what the FP32 pipe of the GMM kernel's roofline_scoring can reach on this
+// device, against the data-sheet figure bench.py divides by.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ffma ffma.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -17,38 +17,18 @@ __global__ void __launch_bounds__(256) k(float *out, int iters, float a, float b
   out[blockIdx.x * blockDim.x + threadIdx.x] = x0 + x1 + x2 + x3 + x4 + x5 + x6 + x7;
 }
 
-// the packed form the GMM kernel uses (fma.rn.f32x2, SASS FFMA2): two lanes per instruction
-__global__ void __launch_bounds__(256) k2(float2 *out, int iters, float a, float b) {
-  unsigned long long x[8];
-  for (int j = 0; j < 8; j++) { float2 v = make_float2(threadIdx.x + j, threadIdx.x - j); x[j] = *reinterpret_cast<unsigned long long *>(&v); }
-  float2 av = make_float2(a, a), bv = make_float2(b, b);
-  const unsigned long long A = *reinterpret_cast<unsigned long long *>(&av), B = *reinterpret_cast<unsigned long long *>(&bv);
-  for (int i = 0; i < iters; i++) {
-#pragma unroll
-    for (int u = 0; u < 16; u++) {
-#pragma unroll
-      for (int j = 0; j < 8; j++) asm volatile("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(x[j]) : "l"(A), "l"(B));
-    }
-  }
-  unsigned long long s = 0; for (int j = 0; j < 8; j++) s ^= x[j];
-  out[blockIdx.x * blockDim.x + threadIdx.x] = *reinterpret_cast<float2 *>(&s);
-}
-
 int main() {
   int sms = 0, khz = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0); cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
   const int blocks = sms * 8, iters = 4096;
-  float *o; cudaMalloc(&o, sizeof(float2) * blocks * 256);
+  float *o; cudaMalloc(&o, sizeof(float) * blocks * 256);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-  double best1 = 0, best2 = 0;
+  double best1 = 0;
   for (int rep = 0; rep < 5; rep++) {
     cudaEventRecord(e0); k<<<blocks, 256>>>(o, iters, 0.999f, 0.001f); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
     const double tf = 2.0 * 8 * 16 * (double)iters * blocks * 256 / (ms * 1e-3) / 1e12; if (tf > best1) best1 = tf;
-    cudaEventRecord(e0); k2<<<blocks, 256>>>(reinterpret_cast<float2 *>(o), iters, 0.999f, 0.001f); cudaEventRecord(e1); cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-    const double tf2 = 2.0 * 2 * 8 * 16 * (double)iters * blocks * 256 / (ms * 1e-3) / 1e12; if (tf2 > best2) best2 = tf2;
   }
-  printf("{\"ffma_tflops\": %.2f, \"ffma2_tflops\": %.2f, \"sms\": %d, \"clock_mhz\": %d, \"how\": \"tools/ubench/ffma.cu: 8 independent FFMA (FFMA2) chains per thread, %d blocks x 256 threads, best of 5, CUDA events\"}\n",
-         best1, best2, sms, khz / 1000, blocks);
+  printf("{\"ffma_tflops\": %.2f, \"sms\": %d, \"clock_mhz\": %d, \"how\": \"tools/ubench/ffma.cu: 8 independent FFMA chains per thread, %d blocks x 256 threads, best of 5, CUDA events\"}\n",
+         best1, sms, khz / 1000, blocks);
   return cudaGetLastError() != cudaSuccess;
 }

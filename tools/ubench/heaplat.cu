@@ -1,5 +1,5 @@
-// heaplat.cu -- micro-benchmark: what does one level of the single-thread heap sift cost on sm_100a?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o heaplat heaplat.cu ; run on a B200.
+// heaplat.cu -- micro-benchmark: what does one level of the single-thread heap sift cost on sm_90a?
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o heaplat heaplat.cu ; run on an H100.
 // Each variant walks root->leaf paths of a 4096-entry (id,score) heap in shared memory, ITER times, and
 // reports cycles per level (clock64 around the loop, thread 0 of a 256-thread block, others at a barrier).
 #include <cstdio>
@@ -114,7 +114,7 @@ int main() {
   cudaMalloc(&d, N * 4); cudaMemcpy(d, h, N * 4, cudaMemcpyHostToDevice);
   cudaMalloc(&o, sizeof(ho));
   const int iters = 2000;
-  for (int blocks : {1, 148, 592}) {
+  for (int blocks : {1, 132, 528}) {
     for (int v = 0; v < 6; v++) {
       for (int rep = 0; rep < 2; rep++) {
         switch (v) {

@@ -1,6 +1,6 @@
 // heapx.cu -- micro-benchmark of the beam-cut extraction replay on a realistic heap (n=2400 random scores,
 // 800 extractions, loser cut at the 800th largest).  Variants isolate what a level / an extraction costs.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o heapx heapx.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o heapx heapx.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -361,11 +361,12 @@ int main() {
     for (int x = 0; x < extract; x++) { int s = a[m]; ref.push_back(a[1]); a[m] = a[1]; m--; int parent = 1, child;
       while ((child = parent * 2) <= m) { if (child < m && val(a[child]) < val(a[child + 1])) child++; if (val(s) >= val(a[child])) break; a[parent] = a[child]; parent = child; }
       a[parent] = s; } }
-  unsigned long long *d, *o; long long *r, hr[2 * 592];
+  constexpr int WAVE = 4 * 132;   // one resident wave of beam blocks on an H100: 4 per SM
+  unsigned long long *d, *o; long long *r, hr[2 * WAVE];
   cudaMalloc(&d, sizeof(unsigned long long) * (MAXT + 4)); cudaMemcpy(d, h.data(), sizeof(unsigned long long) * (MAXT + 4), cudaMemcpyHostToDevice);
-  cudaMalloc(&o, sizeof(unsigned long long) * 1024 * 592); cudaMalloc(&r, sizeof(hr));
+  cudaMalloc(&o, sizeof(unsigned long long) * 1024 * WAVE); cudaMalloc(&r, sizeof(hr));
   std::vector<unsigned long long> ho(1024);
-  for (int blocks : {1, 592}) for (int mode = 0; mode < 3; mode++) {
+  for (int blocks : {1, WAVE}) for (int mode = 0; mode < 3; mode++) {
     const int nt = 4000;
     for (int rep = 0; rep < 2; rep++) {
       if (mode == 0) kfloor<0><<<blocks, 256>>>(d, n, nt, r); else if (mode == 1) kfloor<1><<<blocks, 256>>>(d, n, nt, r); else kfloor<2><<<blocks, 256>>>(d, n, nt, r);
@@ -375,7 +376,7 @@ int main() {
     double sfl = 0; for (int b = 0; b < blocks; b++) sfl += (double)hr[2 * b];
     printf("blocks %3d tick floor mode %d: %.1f cycles/tick\n", blocks, mode, sfl / blocks / nt);
   }
-  for (int blocks : {1, 592}) {
+  for (int blocks : {1, WAVE}) {
     for (int v : {5, 14, 18, 19}) {
       for (int rep = 0; rep < 2; rep++) {
         switch (v) {
