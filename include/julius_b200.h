@@ -148,10 +148,11 @@ int jb200_decoder_last_timing(jb200_decoder *d, float ms[4]);
 int jb200_decoder_sync_timing(jb200_decoder *d);
 /* bytes moved device->host by the last fetch (results + atoms + words) */
 int64_t jb200_decoder_last_d2h_bytes(const jb200_decoder *d);
-/* how often (frames, since create) the beam cut had to fall back to the plain sequential replay (0 unless forced) */
+/* how often (frames, since create) the beam cut fell back to the plain sequential replay.  Always 0: the cut has no
+ * such fall-back; the function stays for ABI compatibility */
 int64_t jb200_decoder_misspeculations(jb200_decoder *d);
-/* beam-cut replay counters since create: out[0] fall-backs to the plain sequential loop, out[1] replay ticks (tree
- * levels with the single-thread replay), out[2] extractions replayed */
+/* beam-cut replay counters since create: out[0] fall-backs to the plain sequential loop (always 0, as above),
+ * out[1] replay ticks, out[2] extractions replayed */
 int jb200_decoder_heap_stats(jb200_decoder *d, int64_t out[3]);
 /* beam cuts that select the top of the token set (sort_token_upward) since create: out[0] how many,
  * out[1] how many of them were answered by the closed form (score, pre-order position) instead of a replay */

@@ -27,13 +27,10 @@ def up_to_date() -> bool:
     return all(os.path.getmtime(d) <= t for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False, variant: str = "", defines=()) -> str:
-    """variant/defines: an experiment build  libjb200_<variant>.so  compiled with extra -D flags (select it with
-    JB200_LIB=...); the default build is what ships."""
-    lib = LIB if not variant else os.path.join(HERE, f"libjb200_{variant}.so")
-    if not variant and not force and up_to_date():
+def build(force: bool = False, verbose: bool = False) -> str:
+    if not force and up_to_date():
         return LIB
-    objdir = os.path.join(HERE, "csrc", "_obj" + ("_" + variant if variant else ""))
+    objdir = os.path.join(HERE, "csrc", "_obj")
     os.makedirs(objdir, exist_ok=True)
     objs = []
     procs = []
@@ -42,7 +39,7 @@ def build(force: bool = False, verbose: bool = False, variant: str = "", defines
         objs.append(obj)
         # the beam kernel's float decisions must not be FMA-contracted
         extra = ["--fmad=false"] if os.path.basename(src) in ("beam.cu",) else []
-        cmd = [NVCC, *FLAGS, *extra, *defines, "-I", os.path.join(ROOT, "include"), "-c", src, "-o", obj]
+        cmd = [NVCC, *FLAGS, *extra, "-I", os.path.join(ROOT, "include"), "-c", src, "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     log = []
     for src, p in procs:
@@ -55,11 +52,10 @@ def build(force: bool = False, verbose: bool = False, variant: str = "", defines
         f.write("\n".join(log))
     if verbose:
         print("\n".join(log))
-    subprocess.run([NVCC, "-shared", "-o", lib, *objs, *GENCODE], check=True)
-    return lib
+    subprocess.run([NVCC, "-shared", "-o", LIB, *objs, *GENCODE], check=True)
+    return LIB
 
 
 if __name__ == "__main__":
     args = sys.argv[1:]
-    variant = args[args.index("--variant") + 1] if "--variant" in args else ""
-    print(build(force="--force" in args, verbose="-v" in args, variant=variant, defines=[a for a in args if a.startswith("-D")]))
+    print(build(force="--force" in args, verbose="-v" in args))

@@ -12,8 +12,7 @@ import numpy as np
 from . import desc as D
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# JB200_LIB (the variable the C plugin and the beam shim honour too) selects another build of the library, e.g. an
-# experiment variant made by `python -m julius_b200.build --variant NAME -DFLAG=1`
+# JB200_LIB (the variable the C plugin and the beam shim honour too) selects another build of the library
 LIBPATH = os.environ.get("JB200_LIB") or os.path.join(HERE, "libjb200.so")
 
 GMM_EXACT, GMM_FAST = 0, 1

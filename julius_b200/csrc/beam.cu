@@ -23,10 +23,11 @@
 //   * inter-word transitions into the "isolated" roots are pre-reduced per root over the frame's
 //     word-end tokens (max is associative; first/winner seqs are carried along); the per-last-word
 //     bigram rows the reference caches lazily (iw_sc_cache) are tabulated once at create time;
-//   * the beam cut replays the reference's heap select exactly: bottom-up heap construction is
-//     level-parallel (siftdowns of one level touch disjoint subtrees), the extractions are
-//     replayed by one thread on a shared-memory heap (heap_extract_fast) while the other warps
-//     reset the per-node slots for the next frame.
+//   * the beam cut reproduces the reference's heap select exactly (beam_cut): bottom-up heap
+//     construction is level-parallel (siftdowns of one level touch disjoint subtrees), the
+//     extraction order comes from a closed form (heap_select_closed) or from a replay by one warp
+//     with up to 16 extractions in flight (heap_pipe.cuh), and the other warps reset the per-node
+//     slots for the next frame meanwhile.
 // All frames of an utterance run inside one kernel launch; tokens, node slots and candidates
 // live in per-utterance global scratch (L2 resident), the sort/heap array in shared memory.
 //
@@ -46,10 +47,7 @@ int gmm_launch_states(jb200_gmm *h, const float *d_feats, int T, float *d_rows, 
                       const int *seg_off, const int *seg_start, int n_seg);
 int gmm_cd_device(const jb200_gmm *h, const int **cd_off, const int **cd_states, int *method, int *nbest);
 
-#ifndef JB200_BEAM_THREADS
-#define JB200_BEAM_THREADS 256
-#endif
-static constexpr int BEAM_THREADS = JB200_BEAM_THREADS;
+static constexpr int BEAM_THREADS = 256;
 static constexpr int NWARP = BEAM_THREADS / 32;
 static constexpr int SEQ_LOCAL_BITS = 18;
 static constexpr unsigned SEQ_LOCAL = 1u << SEQ_LOCAL_BITS;
@@ -120,7 +118,8 @@ struct BeamParams {
   jb200_utt_result *results; int *words;
   long long *prof;            // [n_utts][8] cycle counters per phase, or NULL
   unsigned *bitmask; int *wordpre;   // per-utterance arrival-order bitmask [maxbits/32] and its word prefix counts
-  unsigned long long *misspec_counter; int force_seq_heap, check_heap, no_lose, prof_fine, heap_single, no_closed;
+  unsigned long long *misspec_counter;        // beam-cut counters, see jb200_decoder_create
+  int check_heap;                              // JB200_CHECK_HEAP=1: check every cut against the plain sequential replay
   unsigned long long *lmc; int lmc_bits;      // memo of max_successor_prob, 2^lmc_bits entries (0 = off)
   int maxt, maxc, maxw, maxbits;
   // token sets too large for shared memory (wide beams on large trees): the heap-select array lives in global memory
@@ -130,7 +129,6 @@ struct BeamParams {
   const uint8_t *cp_allowed; const int *init_node; const float *init_lscore; int n_init; float penalty1;
   // chunked launches
   const ChunkDesc *chunk; UttState *state; int interim; int *interim_words;   // [n_utts][MAX_WORDS]
-  int no_reloc;             // JB200_NO_RELOCATE=1: replay the loop whenever the plain closed form's test fails (A/B)
   int atoms_in_place;       // streams: the finalized atoms of utterance u go to atoms_out + atom_off[u] (no batch compaction)
 };
 
@@ -192,23 +190,16 @@ __device__ __forceinline__ float max_successor_prob(const BeamParams &p, int las
   return v;
 }
 
-// a state score is read once per utterance-frame (the row belongs to this utterance alone): JB200_STREAM_HINTS marks
-// these and the last reads of the candidate records evict-first, so that they displace less of what is re-used
-#ifdef JB200_STREAM_HINTS
-#define JB_LD_ROW(p_) __ldcs(p_)
-#else
-#define JB_LD_ROW(p_) __ldg(p_)
-#endif
 // outprob_cd, outprob.c:286-400, evaluated on demand from the frame's state-score row
 __device__ float cdset_score(const BeamParams &p, const float *__restrict__ row, int c) {
   const int b0 = __ldg(p.cd_off + c), n_in = __ldg(p.cd_off + c + 1) - b0;
   if (p.iwcd_method == JB200_IWCD_AVG) {
     float sum = 0.0f; int j = 0;
-    for (int i = 0; i < n_in; i++) { float v = JB_LD_ROW(row + __ldg(p.cd_states + b0 + i)); if (v > JB200_LOG_ZERO) { sum += v; j++; } }
+    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(p.cd_states + b0 + i)); if (v > JB200_LOG_ZERO) { sum += v; j++; } }
     return sum / (float)j;
   } else if (p.iwcd_method == JB200_IWCD_MAX) {
     float mx = JB200_LOG_ZERO;
-    for (int i = 0; i < n_in; i++) { float v = JB_LD_ROW(row + __ldg(p.cd_states + b0 + i)); if (mx < v) mx = v; }
+    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(p.cd_states + b0 + i)); if (mx < v) mx = v; }
     return mx;
   }
   const int maxn = p.iwcd_nbest;
@@ -217,7 +208,7 @@ __device__ float cdset_score(const BeamParams &p, const float *__restrict__ row,
     // largest down (outprob.c:313-318): three registers instead of an indexed array in local memory
     float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY; int n = 0;
     for (int i = 0; i < n_in; i++) {
-      const float v = JB_LD_ROW(row + __ldg(p.cd_states + b0 + i));
+      const float v = __ldg(row + __ldg(p.cd_states + b0 + i));
       if (v <= JB200_LOG_ZERO) continue;
       n++;
       if (v > m0) { m2 = m1; m1 = m0; m0 = v; }
@@ -233,7 +224,7 @@ __device__ float cdset_score(const BeamParams &p, const float *__restrict__ row,
   }
   float mp[CD_NMAX + 1]; int n = 0;
   for (int i = 0; i < n_in; i++) {
-    float prob = JB_LD_ROW(row + __ldg(p.cd_states + b0 + i));
+    float prob = __ldg(row + __ldg(p.cd_states + b0 + i));
     if (prob <= JB200_LOG_ZERO) continue;
     if (n == 0 || prob <= mp[n - 1]) {
       if (n == maxn) continue;
@@ -258,11 +249,11 @@ __device__ float cdset_score(const BeamParams &p, const float *__restrict__ row,
 // outprob_style, outprob_style.c:354-494 with the context resolution tabulated on the host
 __device__ __forceinline__ float outprob_style(const BeamParams &p, const float *__restrict__ row, int out, int last_wid) {
   const int style = (unsigned)out >> 28, ref = out & 0x0fffffff;
-  if (style == JB200_AS_STATE) return JB_LD_ROW(row + ref);
+  if (style == JB200_AS_STATE) return __ldg(row + ref);
   if (style == JB200_AS_LSET) return cdset_score(p, row, ref);
   const int col = (last_wid < 0) ? p.n_ctx : __ldg(p.word_ctx + last_wid);
   const int r = __ldg(p.rset_ctx + (size_t)ref * (p.n_ctx + 1) + col);
-  if (r >= 0) return JB_LD_ROW(row + r);
+  if (r >= 0) return __ldg(row + r);
   return cdset_score(p, row, -r - 1);
 }
 
@@ -479,32 +470,8 @@ __device__ void heap_extract_pipe_global(unsigned long long *A, const int n, con
   ticks_out = ticks; stalls_out = stalls;
 }
 
-__device__ __forceinline__ void lds_pair(unsigned addr, unsigned &x0, unsigned &x1, unsigned &y0, unsigned &y1) {
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x0), "=r"(x1), "=r"(y0), "=r"(y1) : "r"(addr) : "memory");
-}
-__device__ __forceinline__ void lds_one(unsigned addr, unsigned &x0, unsigned &x1) {
-  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(x0), "=r"(x1) : "r"(addr) : "memory");
-}
-__device__ __forceinline__ void sts_one(unsigned addr, unsigned x0, unsigned x1) {
-  asm volatile("st.shared.v2.u32 [%0], {%1,%2};" :: "r"(addr), "r"(x0), "r"(x1) : "memory");
-}
-
-// Fast single-thread extraction replay.  Same comparisons as heap_extract_seq, arranged so that the
-// loop-carried dependence of one tree level is  LDS.128 -> compare -> select next address -> LDS.128 :
-//   * a freed tail slot is overwritten with a sentinel (-inf for the max-heap, +inf for the min-heap) and
-//     so is everything between n+1 and the last child slot (heap_pad_sentinels), which makes both bounds
-//     tests of the reference loop ("child <= n", "child < n") fall out of the value comparisons: a
-//     missing right child never wins, a missing pair stops the sift;
-//   * the children of BOTH possible next parents have known addresses before the comparison resolves, so
-//     the next pair is requested right after the compare, ahead of the stop test (a harmless read when
-//     the sift ends; addresses are clamped to a sentinel pair at the end of the array).  ptxas sinks a
-//     load below the branch when nothing on the exit path reads it, and ld.volatile costs ~50 cycles per
-//     level (tools/ubench/heapx.cu: 97 vs 54 cycles/level), hence the `sink` value that the exit path
-//     folds into the statistics word;
-//   * the extracted roots go to `outv` (k-th extracted at outv[k]) instead of the tail slots.
-// ~45 instead of ~100 cycles per level.  Ends with a barrier.
-// work for the otherwise idle warps during a single-thread extraction replay: reset the per-node slots of the
-// tokens created in this frame (clear_tokens, beam.c:1122, moved ahead of the next frame)
+// work for the otherwise idle warps during an extraction replay: reset the per-node slots of the tokens created in this
+// frame (clear_tokens, beam.c:1122, moved ahead of the next frame)
 struct SlotClear {
   const Tok *tok; int n; SlotView slots;
   __device__ __forceinline__ void run(int first, int stride) const {
@@ -515,6 +482,9 @@ struct SlotClear {
   }
 };
 
+// Freed tail slots and everything between n+1 and the last child slot hold a sentinel (-inf for the max-heap, +inf for
+// the min-heap), and so does the pair (maxt+2, maxt+3): both bounds tests of the reference loop ("child <= n",
+// "child < n") fall out of the value comparisons -- a missing right child never wins, a missing pair stops the sift.
 template <bool MAXHEAP>
 __device__ __forceinline__ void heap_pad_sentinels(unsigned long long *A, const int n, const int maxt) {
   const unsigned long long sent = MAXHEAP ? 0xff800000ull : 0x7f800000ull;
@@ -523,52 +493,49 @@ __device__ __forceinline__ void heap_pad_sentinels(unsigned long long *A, const 
   if (threadIdx.x < 2) A[maxt + 2 + threadIdx.x] = sent;
 }
 
-template <bool MAXHEAP>
-__device__ __forceinline__ unsigned heap_pick(unsigned x0, unsigned y0, unsigned a_left, unsigned a_right, bool &right) {
-  // "child < child+1" (beam.c:1359 / :1425) and the address of the chosen child's own children, one select
-  unsigned r, pr;
-  if (MAXHEAP) asm("{ .reg .pred p; setp.lt.f32 p, %4, %5; selp.u32 %0, %2, %3, p; selp.u32 %1, 1, 0, p; }"
-                   : "=r"(r), "=r"(pr) : "r"(a_right), "r"(a_left), "f"(__uint_as_float(x0)), "f"(__uint_as_float(y0)));
-  else asm("{ .reg .pred p; setp.gt.f32 p, %4, %5; selp.u32 %0, %2, %3, p; selp.u32 %1, 1, 0, p; }"
-           : "=r"(r), "=r"(pr) : "r"(a_right), "r"(a_left), "f"(__uint_as_float(x0)), "f"(__uint_as_float(y0)));
-  right = (pr != 0u);
-  return r;
+// The work areas of the heap select, the same in every beam kernel.  Shared memory: [heap (maxt+4 entries) | offs], or,
+// when the token set is too large for shared memory and the heap lives in global memory (heap_g),
+// [qcap entries: the closed form's sort area and the replay's copy of the heap | offs | copy of the tail slots].
+// offs: 2 x (beam+2) ints that hold the kernels' per-survivor offsets; they are dead during the cut, which keeps its
+// histogram, the closed form's payload and the extracted roots (outv) there.
+extern __shared__ __align__(16) unsigned char beam_smem[];
+struct CutAreas {
+  unsigned long long *heap;             // slot h = heap index h
+  int *offs;
+  unsigned long long *gq; int gqn;      // global heap only: the shared-memory area in front of offs
+  unsigned long long *gtail; int gtn;   // global heap only: the shared-memory copy of the tail slots behind offs
+  __device__ __forceinline__ unsigned long long *outv() const { return reinterpret_cast<unsigned long long *>(offs); }
+};
+__device__ __forceinline__ CutAreas cut_areas(const BeamParams &p) {
+  unsigned long long *const smem_q = reinterpret_cast<unsigned long long *>(beam_smem);
+  CutAreas a;
+  a.heap = p.heap_g ? p.heap_g + (size_t)blockIdx.x * (p.maxt + 4) : smem_q;
+  a.offs = reinterpret_cast<int *>(smem_q + (p.heap_g ? p.qcap : p.maxt + 4));
+  a.gq = p.heap_g ? smem_q : nullptr;
+  a.gqn = p.heap_g ? p.qcap : 0;
+  a.gtail = p.heap_g ? reinterpret_cast<unsigned long long *>(a.offs + 2 * (p.beam + 2)) : nullptr;
+  a.gtn = p.heap_g ? p.beam + 1 : 0;
+  return a;
 }
 
-// one tree level: pair (X0,X1),(Y0,Y1) = children of the parent at `slot`; requests the next pair into N*
-#define JB_HEAP_LEVEL(X0, X1, Y0, Y1, N0, N1, N2, N3)                                                        \
-  {                                                                                                          \
-    const unsigned u = (cur << 1) - hb;                                                                      \
-    bool right;                                                                                              \
-    const unsigned ncur = heap_pick<MAXHEAP>(X0, Y0, min(u, capa), min(u + 16u, capa), right);               \
-    lds_pair(ncur, N0, N1, N2, N3);                      /* speculative: children of the chosen child */     \
-    sink = N0;                                           /* (read on the exit path too, see below) */        \
-    const unsigned c_lo = right ? Y0 : X0, c_hi = right ? Y1 : X1;                                           \
-    levels++;                                                                                                \
-    if (hstop<MAXHEAP>(sv, __uint_as_float(c_lo)) || (MAXHEAP && __uint_as_float(c_lo) < lose_below)) break; \
-    sts_one(slot, c_lo, c_hi);                                                                               \
-    slot = cur + (right ? 8u : 0u);                                                                          \
-    cur = ncur;                                                                                              \
-  }
-
+// Extraction replay of the heap ca.heap[1..n] (sentinel padded): the k-th extracted root goes to outv[k].  Warp 0
+// replays, the other warps run idle_work.  Ends with a barrier.
 template <bool MAXHEAP>
-__device__ void heap_extract_fast(unsigned long long *A, const int n, const int extract, const float lose_below,
-                                  unsigned long long *outv, const int maxt, unsigned long long *stats,
-                                  const SlotClear *idle_work = nullptr, const int single_thread = 0,
-                                  unsigned long long *gcache = nullptr, const int gcache_n = 0,
-                                  unsigned long long *gtail = nullptr, const int gtail_n = 0) {
+__device__ void heap_extract_fast(const CutAreas &ca, const int n, const int extract, const float lose_below, const int maxt,
+                                  unsigned long long *stats, const SlotClear *idle_work = nullptr) {
+  unsigned long long *const A = ca.heap, *const outv = ca.outv(), *const gcache = ca.gq;
   HeapCache hc{nullptr, 0, nullptr, 0, 0};
-  if (!__isShared(A) && gcache && n + 8 <= gcache_n && single_thread != 1) {
+  if (!__isShared(A) && n + 8 <= ca.gqn) {
     // global-memory heap that fits the shared-memory area as a whole (select #1 of a multipath frame, and the smaller
     // frames of a wide beam): replay on a shared-memory copy at shared-memory speed, then write the arrangement back
-    const int lmaxt = (gcache_n - 4) & ~1;
+    const int lmaxt = (ca.gqn - 4) & ~1;
     for (int i = threadIdx.x; i <= n; i += BEAM_THREADS) gcache[i] = A[i];
     heap_pad_sentinels<MAXHEAP>(gcache, n, lmaxt);
     __syncthreads();
     if (threadIdx.x >= 32 && idle_work) idle_work->run((int)threadIdx.x - 32, BEAM_THREADS - 32);
     if (threadIdx.x < 32) {
       unsigned ticks, stalls;
-      heap_extract_pipe_warp6<MAXHEAP, 0>(gcache, n, extract, lose_below, outv, lmaxt, threadIdx.x, ticks, stalls);
+      heap_extract_pipe_warp6<MAXHEAP>(gcache, n, extract, lose_below, outv, lmaxt, threadIdx.x, ticks, stalls);
       if (threadIdx.x == 0) {
         atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
         atomicAdd(stats + 3, (unsigned long long)stalls);
@@ -579,63 +546,29 @@ __device__ void heap_extract_fast(unsigned long long *A, const int n, const int 
     __syncthreads();
     return;
   }
-  if (!__isShared(A) && gcache && gcache_n > 0) {
+  if (!__isShared(A)) {
     // global-memory heap: copy its top levels and its tail into shared memory first (all threads)
-    hc.top = gcache; hc.cs = min(gcache_n, maxt + 4) & ~1;
+    hc.top = gcache; hc.cs = min(ca.gqn, maxt + 4) & ~1;
     for (int i = threadIdx.x; i < hc.cs; i += BEAM_THREADS) gcache[i] = A[i];
-    if (gtail && gtail_n >= extract) {
-      hc.tail = gtail; hc.tail_first = n - extract + 1; hc.tail_n = extract;
-      for (int i = threadIdx.x; i < extract; i += BEAM_THREADS) gtail[i] = A[hc.tail_first + i];
+    if (ca.gtn >= extract) {
+      hc.tail = ca.gtail; hc.tail_first = n - extract + 1; hc.tail_n = extract;
+      for (int i = threadIdx.x; i < extract; i += BEAM_THREADS) ca.gtail[i] = A[hc.tail_first + i];
     }
     __syncthreads();
   }
   if (threadIdx.x >= 32 && idle_work) idle_work->run((int)threadIdx.x - 32, BEAM_THREADS - 32);
-  if (single_thread != 1 || !__isShared(A)) {
-    // warp 0: up to 16 extractions in flight, one tree level per tick each (heap_pipe.cuh)
-    if (threadIdx.x < 32) {
-      unsigned ticks, stalls;
-      if (!__isShared(A)) heap_extract_pipe_global<MAXHEAP>(A, n, extract, lose_below, outv, maxt, hc, ticks, stalls);
-      else
-      if (single_thread == 2) heap_extract_pipe_warp<MAXHEAP>(A, n, extract, lose_below, outv, maxt, threadIdx.x, ticks, stalls);
-      else if (single_thread == 3) heap_extract_pipe_warp4<MAXHEAP, 0>(A, n, extract, lose_below, outv, maxt, threadIdx.x, ticks, stalls);
-      else heap_extract_pipe_warp6<MAXHEAP, 0>(A, n, extract, lose_below, outv, maxt, threadIdx.x, ticks, stalls);
-      if (threadIdx.x == 0) {
-        atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
-        atomicAdd(stats + 3, (unsigned long long)stalls);
-      }
+  // warp 0: up to 16 extractions in flight, one tree level per tick each (heap_pipe.cuh)
+  if (threadIdx.x < 32) {
+    unsigned ticks, stalls;
+    if (!__isShared(A)) heap_extract_pipe_global<MAXHEAP>(A, n, extract, lose_below, outv, maxt, hc, ticks, stalls);
+    else heap_extract_pipe_warp6<MAXHEAP>(A, n, extract, lose_below, outv, maxt, threadIdx.x, ticks, stalls);
+    if (threadIdx.x == 0) {
+      atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
+      atomicAdd(stats + 3, (unsigned long long)stalls);
     }
-    __syncthreads();
-    return;
-  }
-  if (threadIdx.x == 0) {
-    unsigned levels = 0, sink = 0, sinkacc = 0;
-    const unsigned hb = smem_u32(A);
-    const unsigned sent = MAXHEAP ? 0xff800000u : 0x7f800000u;
-    const unsigned capa = hb + (((unsigned)(maxt >> 1) + 1u) << 4);    // pair (maxt+2, maxt+3): always sentinels
-    unsigned mslot = hb + ((unsigned)n << 3);
-    for (int x = 0; x < extract; x++) {
-      unsigned s_lo, s_hi, r_lo, r_hi, x0, x1, y0, y1, z0, z1, w0, w1;
-      lds_one(mslot, s_lo, s_hi);                       // s = A[m]
-      sts_one(mslot, sent, 0u);                         // slot m leaves the heap (before the root's children are read)
-      lds_one(hb + 8u, r_lo, r_hi);                     // root
-      lds_pair(hb + 16u, x0, x1, y0, y1);               // its children
-      mslot -= 8u;
-      outv[x] = ((unsigned long long)r_hi << 32) | r_lo;
-      const float sv = __uint_as_float(s_lo);
-      unsigned slot = hb + 8u, cur = hb + 16u;          // address of the parent slot / of its children pair
-      while (true) {
-        JB_HEAP_LEVEL(x0, x1, y0, y1, z0, z1, w0, w1)
-        JB_HEAP_LEVEL(z0, z1, w0, w1, x0, x1, y0, y1)
-      }
-      sts_one(slot, s_lo, s_hi);
-      sinkacc += sink;
-    }
-    atomicAdd(stats + 1, (unsigned long long)levels); atomicAdd(stats + 2, (unsigned long long)extract);
-    atomicAdd(stats + 3, (unsigned long long)sinkacc);
   }
   __syncthreads();
 }
-#undef JB_HEAP_LEVEL
 
 // ---- closed form of an upward select ------------------------------------------------------------------------------
 // When every sift of the extraction loop ends on a loser (an element that is never extracted) an extraction is a pure
@@ -814,7 +747,7 @@ __device__ __noinline__ int closed_relocate(unsigned long long *keys, const int 
 
 __device__ int heap_select_closed(unsigned long long *heap, const int n, const int need, const float lose_below, const int maxt,
                                   unsigned long long *keys, const int key_cap, unsigned *pay, const int pay_cap,
-                                  int *ordn, int *s_scratch /* [2] shared ints */, const int p_no_reloc = 0) {
+                                  int *ordn, int *s_scratch /* [2] shared ints */) {
   const int tid = threadIdx.x;
   int relocated = 0;
   if (n >= 65536 || maxt >= 65536 || !(lose_below > -INFINITY)) return 0;
@@ -896,7 +829,7 @@ __device__ int heap_select_closed(unsigned long long *heap, const int n, const i
   if (s_scratch[1]) {
     // 3b. a tied tail element may still be in its leaf when the leaf is taken: follow the few re-insertions exactly on the
     //     implicit heap (closed_relocate); warp 0, the others wait
-    if (!can_relocate || p_no_reloc) return 0;
+    if (!can_relocate) return 0;
     if (tid < 32) { const int ok = closed_relocate(keys, nc, n, need, flags, multi, pay, tid); if (tid == 0) s_scratch[1] = ok ? 2 : 1; }
     __syncthreads();
     if (s_scratch[1] != 2) return 0;
@@ -931,6 +864,80 @@ __device__ void interim_best(const BeamParams &p, const int u, const jb200_atom 
 
 // phase cycle accounting (thread 0 only; negligible cost)
 #define PROF_MARK(k) do { if (tid == 0) { long long _n = clock64(); s_prof[k] += _n - s_tprev; s_tprev = _n; } } while (0)
+
+// ---- the beam cut: sort_token_no_order (beam.c:1492-1520) of n > need = beam tokens ------------------------------
+// heap[1..n] holds (token id << 32 | score bits); s_maxkey = fkey of the largest score among them.  Fills ordn[0..need)
+// with the survivors in the reference's order: upward (need < n - need) the extracted maxima, last extracted first;
+// downward what is left of the heap.  The node slots of the n tokens `tn` are dead from here on and are reset for the
+// next frame on the side.  All threads call it; each thread's own ordn entries are written when it returns (no barrier).
+__device__ __forceinline__ void beam_cut(const BeamParams &p, const CutAreas &ca, const int n, const unsigned &s_maxkey,
+                                         const Tok *tn, const SlotView &slots, int *ordn, long long *s_prof, long long &s_tprev) {
+  __shared__ unsigned s_losekey;
+  __shared__ int s_cf[2];
+  const int tid = threadIdx.x;
+  const int need = p.beam, maxt = p.maxt;
+  unsigned long long *const heap = ca.heap, *const outv = ca.outv();
+  const SlotClear sc{tn, n, slots};
+  if (need < n - need) {
+    // lower bound of the need-th largest score from a 1024-bin histogram of the order-preserving keys (bin width ~0.5
+    // in score units, adapted to the magnitude of the best score)
+    constexpr int NB = 1024;
+    int *hist = ca.offs;
+    const int nb = min(NB, 2 * (p.beam + 2));
+    for (int i = tid; i < nb; i += BEAM_THREADS) hist[i] = 0;
+    __syncthreads();
+    const unsigned maxkey = s_maxkey;
+    const int e = (int)((((maxkey & 0x80000000u) ? (maxkey & 0x7fffffffu) : ~maxkey) >> 23) & 0xffu) - 127;
+    const int sh = max(0, min(24, 22 - e));
+    for (int r = tid; r < n; r += BEAM_THREADS) {
+      const unsigned key = fkey(hval(heap[r + 1]));
+      const unsigned bin = min((unsigned)(nb - 1), (maxkey - key) >> sh);
+      atomicAdd(&hist[bin], 1);
+    }
+    __syncthreads();
+    if (tid < 32) {
+      int cum = 0, found = -1;
+      for (int b0 = 0; b0 < nb && found < 0; b0 += 32) {
+        const int v = (b0 + tid < nb) ? hist[b0 + tid] : 0;
+        int x = v;
+        for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, o); if (tid >= o) x += y; }
+        const unsigned hit = __ballot_sync(0xffffffffu, cum + x >= need);
+        if (hit) found = b0 + __ffs(hit) - 1;
+        cum += __shfl_sync(0xffffffffu, x, 31);
+      }
+      if (tid == 0) {
+        unsigned lk = 0u;
+        if (found >= 0 && found < nb - 1) {
+          const unsigned long long drop = (unsigned long long)(found + 1) << sh;
+          lk = (drop < maxkey) ? maxkey - (unsigned)drop : 0u;
+        }
+        s_losekey = lk;
+      }
+    }
+    __syncthreads();
+    const unsigned lk = s_losekey;
+    const float lose_below = (lk == 0u) ? -INFINITY : __uint_as_float((lk & 0x80000000u) ? (lk & 0x7fffffffu) : ~lk);
+    heap_build<true>(heap, n); PROF_MARK(7);
+    // closed form of the extraction order when no re-inserted element can matter (heap_select_closed), else the replay;
+    // the node slots are reset before the sort
+    sc.run(tid, BEAM_THREADS);
+    const int closed = heap_select_closed(heap, n, need, lose_below, maxt, ca.gq ? ca.gq : heap + n + 1, ca.gq ? p.sort_cap : maxt + 3 - n,
+                                          reinterpret_cast<unsigned *>(ca.offs), 2 * (p.beam + 2), ordn, s_cf);
+    if (tid == 0) { atomicAdd(p.misspec_counter + 4, 1ull); if (closed) atomicAdd(p.misspec_counter + 5, 1ull); if (closed == 2) atomicAdd(p.misspec_counter + 6, 1ull); }
+    if (!closed) {
+      heap_pad_sentinels<true>(heap, n, maxt);
+      __syncthreads();
+      heap_extract_fast<true>(ca, n, need, lose_below, maxt, p.misspec_counter);
+      for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(outv[need - 1 - k] >> 32);
+    }
+  } else {
+    // downward: no loser cut, no closed form; the idle warps reset the node slots during the replay
+    heap_pad_sentinels<false>(heap, n, maxt);
+    heap_build<false>(heap, n); PROF_MARK(7);
+    heap_extract_fast<false>(ca, n, n - need, -INFINITY, maxt, p.misspec_counter, &sc);
+    for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
+  }
+}
 
 // finalize_1st_pass (bt_relocate_rw + bt_sort_rw, backtrellis.c:218-267,438-478) + find_1pass_result
 // (beam.c:394-424, :253-301); shared by the normal and the multipath kernel.  All threads call it.
@@ -1081,11 +1088,7 @@ __device__ __forceinline__ void finalize_utt_grammar(const BeamParams &p, const 
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------
-extern __shared__ __align__(16) unsigned char beam_smem[];
-
-#ifndef JB200_BEAM_MINBLOCKS
-#define JB200_BEAM_MINBLOCKS 4
-#endif
+static constexpr int BEAM_MINBLOCKS = 4;
 #define BEAM_KERNEL_NAME beam_kernel
 #define BEAM_GRAMMAR 0
 #include "beam_frames.inc"
@@ -1110,16 +1113,15 @@ extern __shared__ __align__(16) unsigned char beam_smem[];
 // Half B reuses the per-node slots: a token made in half A keeps the slot with firstseq = id - 2^30 (< 0:
 // "exists") and bestkey = (score, seq 0), so later arrivals only replace its content when strictly better.
 template <bool MAXHEAP>
-__device__ __forceinline__ int select_exact(unsigned long long *heap, int n, int need, int *ordn, unsigned long long *outv, int maxt,
-                                            unsigned long long *stats, const int heap_single,
-                                            unsigned long long *gcache, const int gcache_n, unsigned long long *gtail, const int gtail_n) {
+__device__ __forceinline__ int select_exact(const CutAreas &ca, int n, int need, int *ordn, int maxt, unsigned long long *stats) {
   // sort_token_no_order (beam.c:1492-1520) replayed in full; the extracted roots are put back into the
   // tail slots where the in-place algorithm leaves them (k-th extracted at slot n-k).  Returns the first
   // survivor's slot.
+  unsigned long long *const heap = ca.heap, *const outv = ca.outv();
   const int extract = MAXHEAP ? need : n - need;
   heap_pad_sentinels<MAXHEAP>(heap, n, maxt);
   heap_build<MAXHEAP>(heap, n);
-  heap_extract_fast<MAXHEAP>(heap, n, extract, -INFINITY, outv, maxt, stats, nullptr, heap_single, gcache, gcache_n, gtail, gtail_n);
+  heap_extract_fast<MAXHEAP>(ca, n, extract, -INFINITY, maxt, stats);
   for (int k = threadIdx.x; k < extract; k += BEAM_THREADS) heap[n - k] = outv[k];
   __syncthreads();
   const int start = MAXHEAP ? n - need : 0;
@@ -1129,7 +1131,7 @@ __device__ __forceinline__ int select_exact(unsigned long long *heap, int n, int
 
 static constexpr int TOK_EXISTS = 0x40000000;
 
-__global__ void __launch_bounds__(BEAM_THREADS, JB200_BEAM_MINBLOCKS)
+__global__ void __launch_bounds__(BEAM_THREADS, BEAM_MINBLOCKS)
 beam_kernel_mp(const BeamParams p) {
   const int u = blockIdx.x;
   const int tid = threadIdx.x;
@@ -1142,20 +1144,12 @@ beam_kernel_mp(const BeamParams p) {
   const int T = ck.t1;                               // frames so far; the utterance's length when ck_final
   const int MAXT = p.maxt, MAXC = p.maxc, MAXW = p.maxw;
 
-  // shared memory: [heap (MAXT+4 entries) | offs], or, when the heap lives in global memory, [sort area | offs]
-  unsigned long long *const smem_q = reinterpret_cast<unsigned long long *>(beam_smem);
-  unsigned long long *heap = p.heap_g ? p.heap_g + (size_t)blockIdx.x * (MAXT + 4) : smem_q;
-  int *offs = reinterpret_cast<int *>(smem_q + (p.heap_g ? p.qcap : MAXT + 4));
-  int *hist = offs;                                                               // reused by select #2
-  // global-memory heap: the area in front of offs doubles as the replay's copy of the heap's top levels, and a copy of
-  // the tail slots follows offs
-  unsigned long long *const gq = p.heap_g ? smem_q : nullptr;
-  const int gqn = p.heap_g ? p.qcap : 0;
-  unsigned long long *const gtail = p.heap_g ? reinterpret_cast<unsigned long long *>(offs + 2 * (p.beam + 2)) : nullptr;
-  const int gtn = p.heap_g ? p.beam + 1 : 0;
+  const CutAreas ca = cut_areas(p);
+  unsigned long long *const heap = ca.heap;
+  int *const offs = ca.offs;                           // [beam+2] candidate offsets per survivor
   __shared__ int s_warp[NWARP + 1];
-  __shared__ int s_E, s_natoms, s_ns, s_cur, s_overflow, s_found, s_cf[2];
-  __shared__ unsigned s_pmaxkey, s_hmaxkey, s_losekey;
+  __shared__ int s_E, s_natoms, s_ns, s_cur, s_overflow, s_found;
+  __shared__ unsigned s_pmaxkey, s_hmaxkey;
   __shared__ unsigned long long s_webest;
   __shared__ float s_thr;
   __shared__ long long s_outbase;
@@ -1169,7 +1163,6 @@ beam_kernel_mp(const BeamParams p) {
   WEnd *wend = p.wend + (size_t)u * MAXW;
   unsigned *bits = p.bitmask + (size_t)u * (p.maxbits >> 5);
   int *wpre = p.wordpre + (size_t)u * (p.maxbits >> 5);
-  unsigned long long *outv = reinterpret_cast<unsigned long long *>(offs);   // [beam+1] extracted roots; offs is dead during the selects
   const long long a0 = p.atom_off[u];
   const int atom_cap = (int)(p.atom_off[u + 1] - a0);
   jb200_atom *araw = p.atoms_raw + a0;
@@ -1346,8 +1339,8 @@ beam_kernel_mp(const BeamParams p) {
         for (int k = tid; k < ns_a; k += BEAM_THREADS) ordn[k] = k;
       } else {
         ns_a = need;
-        if (need < ncre_a - need) select_exact<true>(heap, ncre_a, need, ordn, outv, MAXT, p.misspec_counter, p.heap_single, gq, gqn, gtail, gtn);
-        else select_exact<false>(heap, ncre_a, need, ordn, outv, MAXT, p.misspec_counter, p.heap_single, gq, gqn, gtail, gtn);
+        if (need < ncre_a - need) select_exact<true>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
+        else select_exact<false>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
       }
     }
     __syncthreads();
@@ -1568,75 +1561,13 @@ beam_kernel_mp(const BeamParams p) {
     PROF_MARK(5);
 
     // ---- B7: heap select #2 (only its survivors' order is observable: loser cut allowed)
-    int ns_new;
-    {
-      const int need = p.beam, rest = ncre - need;
-      if (need >= ncre) {
-        ns_new = ncre;
-        // tindex order = select #1's arrangement, then the new tokens
-        for (int k = tid; k < ns_new; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
-      } else if (need < rest) {
-        ns_new = need;
-        constexpr int NB = 1024;
-        const int nb = min(NB, 2 * (p.beam + 2));
-        for (int i = tid; i < nb; i += BEAM_THREADS) hist[i] = 0;
-        __syncthreads();
-        const unsigned maxkey = s_hmaxkey;
-        const int e = (int)((((maxkey & 0x80000000u) ? (maxkey & 0x7fffffffu) : ~maxkey) >> 23) & 0xffu) - 127;
-        const int sh = max(0, min(24, 22 - e));
-        for (int r = tid; r < ncre; r += BEAM_THREADS) {
-          const unsigned key = fkey(hval(heap[r + 1]));
-          const unsigned bin = min((unsigned)(nb - 1), (maxkey - key) >> sh);
-          atomicAdd(&hist[bin], 1);
-        }
-        __syncthreads();
-        if (tid < 32) {
-          int cum = 0, found = -1;
-          for (int b0 = 0; b0 < nb && found < 0; b0 += 32) {
-            const int v = (b0 + tid < nb) ? hist[b0 + tid] : 0;
-            int x = v;
-            for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, o); if (tid >= o) x += y; }
-            const unsigned hit = __ballot_sync(0xffffffffu, cum + x >= need);
-            if (hit) found = b0 + __ffs(hit) - 1;
-            cum += __shfl_sync(0xffffffffu, x, 31);
-          }
-          if (tid == 0) {
-            unsigned lk = 0u;
-            if (found >= 0 && found < nb - 1) {
-              const unsigned long long drop = (unsigned long long)(found + 1) << sh;
-              lk = (drop < maxkey) ? maxkey - (unsigned)drop : 0u;
-            }
-            s_losekey = lk;
-          }
-        }
-        __syncthreads();
-        const unsigned lk = s_losekey;
-        const float lose_below = (lk == 0u || p.no_lose) ? -INFINITY : __uint_as_float((lk & 0x80000000u) ? (lk & 0x7fffffffu) : ~lk);
-        heap_build<true>(heap, ncre); PROF_MARK(7);
-        const SlotClear sc{tn, ncre, slots};
-        slots_clean = true;
-        int closed = 0;
-        if (!p.no_closed) {
-          sc.run((int)threadIdx.x, BEAM_THREADS);
-          closed = heap_select_closed(heap, ncre, need, lose_below, MAXT, p.heap_g ? smem_q : heap + ncre + 1, p.heap_g ? p.sort_cap : MAXT + 3 - ncre,
-                                      reinterpret_cast<unsigned *>(offs), 2 * (p.beam + 2), ordn, s_cf, p.no_reloc);
-          if (tid == 0) { atomicAdd(p.misspec_counter + 4, 1ull); if (closed) atomicAdd(p.misspec_counter + 5, 1ull); if (closed == 2) atomicAdd(p.misspec_counter + 6, 1ull); }
-        }
-        if (!closed) {
-          heap_pad_sentinels<true>(heap, ncre, MAXT);
-          __syncthreads();
-          heap_extract_fast<true>(heap, ncre, need, lose_below, outv, MAXT, p.misspec_counter, p.no_closed ? &sc : nullptr, p.heap_single, gq, gqn, gtail, gtn);
-          for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(outv[need - 1 - k] >> 32);
-        }
-      } else {
-        ns_new = need;
-        heap_pad_sentinels<false>(heap, ncre, MAXT);
-        heap_build<false>(heap, ncre); PROF_MARK(7);
-        const SlotClear sc{tn, ncre, slots};
-        slots_clean = true;
-        heap_extract_fast<false>(heap, ncre, rest, -INFINITY, outv, MAXT, p.misspec_counter, &sc, p.heap_single, gq, gqn, gtail, gtn);
-        for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
-      }
+    const int ns_new = min(ncre, p.beam);
+    if (ncre <= p.beam) {
+      // tindex order = select #1's arrangement, then the new tokens
+      for (int k = tid; k < ns_new; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
+    } else {
+      beam_cut(p, ca, ncre, s_hmaxkey, tn, slots, ordn, s_prof, s_tprev);
+      slots_clean = true;
     }
     PROF_MARK(6);
     if (tid == 0) {
@@ -1710,9 +1641,8 @@ struct jb200_decoder {
   int atoms_per_frame = 64;
   BeamParams P{};
   std::vector<void *> dev_allocs;
-  // read-only tables shared by all utterances (tree, LM, inter-word table, bigram memo) sit in ONE allocation (one
-  // contiguous range for an optional L2 access-policy window, see jb200_decoder_create)
-  char *arena = nullptr; size_t arena_size = 0, arena_used = 0; bool l2_window = false;
+  // read-only tables shared by all utterances (tree, LM, inter-word table, bigram memo) sit in ONE allocation
+  char *arena = nullptr; size_t arena_size = 0, arena_used = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[5]{};
   // batch buffers
@@ -1791,7 +1721,6 @@ static int dev_alloc(jb200_decoder *d, size_t n, Tp **dst) {
 extern "C" void jb200_decoder_destroy(jb200_decoder *d) {
   if (!d) return;
   cudaSetDevice(d->device);
-  if (d->l2_window) cudaCtxResetPersistingL2Cache();
   for (void *p : d->dev_allocs) cudaFree(p);
   if (d->h_results) cudaFreeHost(d->h_results);
   if (d->h_atoms) cudaFreeHost(d->h_atoms);
@@ -1846,13 +1775,14 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
 
   BeamParams &P = d->P;
   const int n = t->n_nodes;
+  // bigram-factoring memo, 2^21 entries: keys are (word id, successor slot) packed 16+16, so it needs both below 65535
+  const int lmc_bits = (t->n_words >= 65535 || t->n_scword >= 65535) ? 0 : 21;
   {
     // shared read-only tables: nodes 32 B, arcs 8 B, context table, inter-word table, bigram memo, LM arrays (+ slack)
-    const int lmc_bits_est = (t->n_words >= 65535 || t->n_scword >= 65535) ? 0 : 21;
     size_t est = (size_t)n * 32 + (size_t)t->n_arcs * 8 * 3 + (size_t)t->n_rset * (t->n_ctx + 1) * 4 + (size_t)t->n_words * 32 +
-                 (size_t)t->n_words * std::max(t->n_iso, 1) * (grammar ? 1 : 4) + ((size_t)8 << lmc_bits_est) +
+                 (size_t)t->n_words * std::max(t->n_iso, 1) * (grammar ? 1 : 4) + ((size_t)8 << lmc_bits) +
                  (size_t)t->lm_nvocab * 16 + (size_t)t->lm_nbigram * 8 + (size_t)(t->n_iso + t->n_shared + t->n_fscore + t->n_scword) * 16 + (4u << 20);
-    if (getenv("JB200_NO_ARENA") == nullptr && cudaMalloc(&d->arena, est) == cudaSuccess) { d->arena_size = est; d->dev_allocs.push_back(d->arena); }
+    if (cudaMalloc(&d->arena, est) == cudaSuccess) { d->arena_size = est; d->dev_allocs.push_back(d->arena); }
     else { d->arena = nullptr; cudaGetLastError(); }
   }
   // Node numbering.  The host numbers the nodes word by word (a word's own nodes are consecutive), so the ~2400 nodes a
@@ -1861,21 +1791,19 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   // are not observable outside the decoder, so the tree is renumbered breadth-first from the roots (roots in their list
   // order, then level by level): the slots and node records a frame touches become a few dense ranges -- 3.4x fewer
   // slot lines, 2.1x fewer node-record lines per frame on the 20k-word tree (tools/node_locality.py).  `next_a` no longer
-  // leads to id+1, so the record carries the successor explicitly.  JB200_NO_RENUMBER=1 keeps the host's numbering.
+  // leads to id+1, so the record carries the successor explicitly.
   std::vector<int> perm(n), inv(n);
   {
     std::vector<int> order; order.reserve(n);
     std::vector<char> seen(n, 0);
     auto push = [&](int x) { if (x >= 0 && x < n && !seen[x]) { seen[x] = 1; order.push_back(x); } };
-    if (getenv("JB200_NO_RENUMBER") == nullptr || atoi(getenv("JB200_NO_RENUMBER")) == 0) {
-      for (int i = 0; i < t->n_iso; i++) push(t->iso_node[i]);
-      for (int i = 0; i < t->n_shared; i++) push(t->shared_node[i]);
-      if (grammar) for (int i = 0; i < t->n_init; i++) push(t->init_node[i]);
-      for (size_t q = 0; q < order.size(); q++) {
-        const int x = order[q];
-        if (t->next_a[x] != JB200_LOG_ZERO) push(x + 1);
-        for (int k = t->arc_off[x]; k < t->arc_off[x + 1]; k++) push(t->arc_to[k]);
-      }
+    for (int i = 0; i < t->n_iso; i++) push(t->iso_node[i]);
+    for (int i = 0; i < t->n_shared; i++) push(t->shared_node[i]);
+    if (grammar) for (int i = 0; i < t->n_init; i++) push(t->init_node[i]);
+    for (size_t q = 0; q < order.size(); q++) {
+      const int x = order[q];
+      if (t->next_a[x] != JB200_LOG_ZERO) push(x + 1);
+      for (int k = t->arc_off[x]; k < t->arc_off[x + 1]; k++) push(t->arc_to[k]);
     }
     for (int x = 0; x < n; x++) push(x);                       // whatever the roots do not reach keeps its relative order
     for (int i = 0; i < n; i++) { perm[order[i]] = i; inv[i] = order[i]; }
@@ -1995,7 +1923,6 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   // 20k-word tree: 4.6*beam at -b 800 (of which startnum = 1375 root tokens), 4.7*beam at -b 4000.  The array lives
   // in shared memory, and what it takes is lost to L1 (5*beam+startnum at -b 800 costs 30 % of the kernel's speed).
   int maxt = (std::max(4 * t->beam_width + t->n_start, 5 * t->beam_width) + 64 + 3) & ~3;
-  if (const char *e = getenv("JB200_MAXT")) maxt = (std::max(atoi(e), 64) + 3) & ~3;
   // Where the heap-select array lives.  Shared memory as long as one block's share fits; a wide beam on a large tree
   // (-b 4000 on the 60k-word multipath tree creates up to 8.5 x beam tokens a frame) goes to global memory instead,
   // with room for 9 x beam + startnum tokens, and shared memory keeps only the closed form's sort area.
@@ -2003,20 +1930,18 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   int smem_limit = 0;
   TRYC(cudaDeviceGetAttribute(&smem_limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->device));
   smem_limit -= 2048;                                       // static shared variables of the kernels
-  bool heap_global = (size_t)(maxt + 4) * 8 + offs_bytes > (size_t)smem_limit / 2;   // would leave one block per SM
-  if (const char *e = getenv("JB200_HEAP_GLOBAL")) heap_global = atoi(e) != 0;
+  const bool heap_global = (size_t)(maxt + 4) * 8 + offs_bytes > (size_t)smem_limit / 2;   // would leave one block per SM
   P.heap_g = nullptr; P.sort_cap = 0; P.qcap = 0;
   if (heap_global) {
-    if (!getenv("JB200_MAXT")) maxt = std::min(65000, (std::max(maxt, 9 * t->beam_width + t->n_start) + 3) & ~3);
+    maxt = std::min(65000, (std::max(maxt, 9 * t->beam_width + t->n_start) + 3) & ~3);
     int sc = 1024; while (sc < 2 * t->beam_width && sc < 16384) sc <<= 1;       // candidates = beam + one histogram bin
     const size_t tail_bytes = (size_t)(t->beam_width + 2) * 8;                   // the replay's copy of the tail slots
     if ((size_t)sc * 8 + offs_bytes + tail_bytes > (size_t)smem_limit) { set_error("beam width %d needs more shared memory than the device has", t->beam_width); jb200_decoder_destroy(d); return JB200_ERR_UNSUPPORTED; }
     P.sort_cap = sc;
     // what is left of shared memory holds the top levels of the heap during a replay (one block per SM: the replay is all
-    // that matters at these beam widths); JB200_HEAP_CACHE=0 keeps only the sort area (two blocks per SM)
+    // that matters at these beam widths)
     int qc = sc;
-    if (!getenv("JB200_HEAP_CACHE") || atoi(getenv("JB200_HEAP_CACHE")) != 0)
-      while ((size_t)qc * 2 * 8 + offs_bytes + tail_bytes <= (size_t)smem_limit && qc * 2 <= ((maxt + 4) | 1023) + 1) qc <<= 1;
+    while ((size_t)qc * 2 * 8 + offs_bytes + tail_bytes <= (size_t)smem_limit && qc * 2 <= ((maxt + 4) | 1023) + 1) qc <<= 1;
     P.qcap = qc;
     TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_g));
   }
@@ -2033,27 +1958,17 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   P.maxbits = (P.maxc + std::min(P.maxw, 256) * n_isoent + std::max(t->n_shared, P.n_sharc) + 63) & ~31;
   TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.bitmask));
   TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.wordpre));
-  TRY(dev_alloc(d, 8, &P.misspec_counter));        // [0] mis-speculations, [1] replay ticks (levels), [2] extractions, [3] held-back starts, [4] upward selects, [5] of which closed form
+  // beam-cut counters: [0] fall-backs to the plain sequential replay (there are none: always 0), [1] replay ticks,
+  // [2] extractions replayed, [3] held-back starts, [4] upward selects, [5] of which closed form, [6] of which with relocations
+  TRY(dev_alloc(d, 8, &P.misspec_counter));
   TRYC(cudaMemset(P.misspec_counter, 0, 8 * sizeof(unsigned long long)));
-  P.force_seq_heap = getenv("JB200_FORCE_SEQ_HEAP") ? atoi(getenv("JB200_FORCE_SEQ_HEAP")) : 0;
   P.check_heap = getenv("JB200_CHECK_HEAP") ? atoi(getenv("JB200_CHECK_HEAP")) : 0;
-  {
-    // bigram-factoring memo: keys are (word id, successor slot) packed 16+16, so it needs both below 65535
-    int bits = getenv("JB200_LMCACHE_BITS") ? atoi(getenv("JB200_LMCACHE_BITS")) : 21;
-    if (t->n_words >= 65535 || t->n_scword >= 65535 || bits < 8) bits = 0;
-    if (bits > 26) bits = 26;
-    P.lmc_bits = bits; P.lmc = nullptr;
-    if (bits > 0) {
-      TRY(dev_alloc_shared(d, (size_t)1 << bits, &P.lmc));
-      TRYC(cudaMemsetAsync(P.lmc, 0xff, sizeof(unsigned long long) << bits, d->stream));
-    }
+  P.lmc_bits = lmc_bits; P.lmc = nullptr;
+  if (lmc_bits > 0) {
+    TRY(dev_alloc_shared(d, (size_t)1 << lmc_bits, &P.lmc));
+    TRYC(cudaMemsetAsync(P.lmc, 0xff, sizeof(unsigned long long) << lmc_bits, d->stream));
   }
   P.chunk = nullptr; P.state = nullptr; P.interim = 0; P.interim_words = nullptr; P.atoms_in_place = 0;
-  P.no_reloc = getenv("JB200_NO_RELOCATE") ? atoi(getenv("JB200_NO_RELOCATE")) : 0;
-  P.prof_fine = getenv("JB200_PROF_FINE") ? atoi(getenv("JB200_PROF_FINE")) : 0;   // extra barrier: slot 4 = word-internal expansion alone
-  P.no_lose = getenv("JB200_NO_LOSER_CUT") ? atoi(getenv("JB200_NO_LOSER_CUT")) : 0;
-  P.no_closed = getenv("JB200_NO_CLOSED_FORM") ? atoi(getenv("JB200_NO_CLOSED_FORM")) : 0;   // 1: always replay the extraction loop
-  P.heap_single = getenv("JB200_HEAP_SINGLE") ? atoi(getenv("JB200_HEAP_SINGLE")) : 0;   // 1: the single-thread replay, 2: the readable pipelined loop, 3: the C++ form of the shipped loop (A/B timing)
   {
     size_t tot = (size_t)max_utts * n;
     fill_slots_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(P.slots, tot);
@@ -2108,25 +2023,6 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
     TRYC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BEAM_THREADS, d->smem_bytes));
     TRYC(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d->device));
     d->resident = per_sm * sms;
-  }
-  // Opt-in (JB200_L2_WINDOW=1): an L2 access-policy window that keeps the shared tables resident (persisting hits, streaming
-  // misses).  Off by default: the set-aside competes with the per-utterance work areas for L2.
-  if (d->arena && d->arena_used > 0 && getenv("JB200_L2_WINDOW") != nullptr && atoi(getenv("JB200_L2_WINDOW")) != 0) {
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, d->device) == cudaSuccess && prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {
-      const size_t win = std::min<size_t>(d->arena_used, (size_t)prop.accessPolicyMaxWindowSize);
-      const size_t carve = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, win);
-      if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve) == cudaSuccess) {
-        cudaStreamAttrValue av{};
-        av.accessPolicyWindow.base_ptr = d->arena;
-        av.accessPolicyWindow.num_bytes = win;
-        av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)win);
-        av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        d->l2_window = (cudaStreamSetAttribute(d->stream, cudaStreamAttributeAccessPolicyWindow, &av) == cudaSuccess);
-      }
-    }
-    cudaGetLastError();
   }
   TRYC(cudaStreamSynchronize(d->stream));
 #undef TRY

@@ -17,10 +17,10 @@
 //   * the only other coupling is the tail slot an extraction takes its s from (and retires):  an older extraction
 //     whose hole sits on an ancestor of that slot, or on the slot, may still compare against its content or end its
 //     own sift there.  The new extraction waits until no hole in flight is on that root path (decided on the holes
-//     as they are before the tick's move, which only errs towards waiting).  With the loser cut of a max-heap select
-//     (a sift stops at a child below `lose_below`, a lower bound of the smallest score that can be extracted) a
-//     tail slot holding a loser is never read for a decision that matters and never becomes a hole, and a loser
-//     stays a loser, so those starts -- 97 % of them on the 20k-word workload -- need no check at all.
+//     as they are after the tick's move).  With the loser cut of a max-heap select (a sift stops at a child below
+//     `lose_below`, a lower bound of the smallest score that can be extracted) a tail slot holding a loser is never read
+//     for a decision that matters and never becomes a hole, and a loser stays a loser, so those starts -- 97 % of them
+//     on the 20k-word workload -- need no check at all.
 // tools/heapsim.cpp runs exactly this schedule on the CPU against the plain loop (tests/test_heapsim.py).
 // 1613 ticks for 800 extractions out of 2470 on the 20k-word workload (tools/heapstat.cpp on a real decode).
 #pragma once
@@ -34,91 +34,8 @@ __device__ __forceinline__ unsigned hp_smem_u32(const void *p) {
   asm volatile("{ .reg .u64 t; cvta.to.shared.u64 t, %1; cvt.u32.u64 %0, t; }" : "=r"(r) : "l"(p));
   return r;
 }
-__device__ __forceinline__ void hp_lds_pair(unsigned addr, unsigned &x0, unsigned &x1, unsigned &y0, unsigned &y1) {
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x0), "=r"(x1), "=r"(y0), "=r"(y1) : "r"(addr) : "memory");
-}
 __device__ __forceinline__ void hp_lds_one(unsigned addr, unsigned &x0, unsigned &x1) {
   asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(x0), "=r"(x1) : "r"(addr) : "memory");
-}
-__device__ __forceinline__ void hp_sts_one(unsigned addr, unsigned x0, unsigned x1) {
-  asm volatile("st.shared.v2.u32 [%0], {%1,%2};" :: "r"(addr), "r"(x0), "r"(x1) : "memory");
-}
-
-// Called by the 32 threads of one warp (lane = 0..31).  A: heap entries (low word = fp32 score bits, high word = token
-// id), slot h = heap index h, sentinel padded; n: heap size; outv[k] = k-th extracted root, k = 0..extract (the last
-// entry is what would be extracted next).  Returns the number of ticks / stalled ticks through the pointers (lane 0).
-template <bool MAXHEAP>
-__device__ __forceinline__ void heap_extract_pipe_warp(unsigned long long *A, const int n, const int extract, const float lose_below,
-                                                       unsigned long long *outv, const int maxt, const unsigned lane,
-                                                       unsigned &ticks_out, unsigned &stalls_out) {
-  constexpr int NL = 16;                                   // extraction x is owned by lane x mod NL
-  constexpr unsigned FULL = 0xffffffffu;
-  const unsigned hb = hp_smem_u32(A);
-  const unsigned sent = MAXHEAP ? 0xff800000u : 0x7f800000u;
-  const unsigned capa = hb + (((unsigned)(maxt >> 1) + 1u) << 4);     // pair (maxt+2, maxt+3): always sentinels
-  const unsigned root = hb + 8u;
-  bool act = false;
-  unsigned slot = capa, cur = capa;                        // hole / its children pair; idle lanes read the sentinel pair
-  unsigned s_lo = sent, s_hi = 0u;
-  int my_x = 0, next_x = 0, wait = 0;
-  unsigned ticks = 0, stalls = 0;
-  unsigned nxt_lo, nxt_hi;                                 // content of the tail slot the next extraction will take
-  hp_lds_one(hb + ((unsigned)n << 3), nxt_lo, nxt_hi);
-  if (lane == 0 && extract > 0) outv[0] = A[1];
-  while (true) {
-    // (1) children pair of the hole
-    unsigned x0, x1, y0, y1;
-    hp_lds_pair(cur, x0, x1, y0, y1);
-    // (2) may the next extraction start?  (all of this sits in the shadow of the load)
-    bool start_me = false;
-    if (next_x < extract) {
-      if (--wait <= 0) {
-        const unsigned ms = (unsigned)(n - next_x);
-        const unsigned ln = (unsigned)next_x & (NL - 1);
-        bool blocks = act && (lane == ln);
-        const bool loser = MAXHEAP && (__uint_as_float(nxt_lo) < lose_below);
-        if (!loser) {
-          const unsigned h = (slot - hb) >> 3;             // hole index (idle lanes: a slot beyond every tail slot)
-          const int dh = 31 - __clz(h), dms = 31 - __clz(ms);
-          blocks = blocks || (act && dms >= dh && (ms >> (dms - dh)) == h);
-        }
-        if (!__any_sync(FULL, blocks)) {
-          start_me = (lane == ln);
-          if (start_me) {
-            const unsigned ma = hb + (ms << 3);
-            hp_lds_one(ma, s_lo, s_hi);                    // s = A[m]
-            hp_sts_one(ma, sent, 0u);                      // slot m leaves the heap
-            my_x = next_x;
-          }
-          next_x++; wait = 2;
-          hp_lds_one(hb + ((unsigned)(n - next_x) << 3), nxt_lo, nxt_hi);
-        } else stalls++;
-      }
-    } else if (!__any_sync(FULL, act)) break;
-    ticks++;
-    // (3) fill the hole, move one level down or end
-    {
-      const float sv = __uint_as_float(s_lo);
-      const bool right = MAXHEAP ? (__uint_as_float(x0) < __uint_as_float(y0)) : (__uint_as_float(x0) > __uint_as_float(y0));
-      const unsigned c_lo = right ? y0 : x0, c_hi = right ? y1 : x1;
-      const float cv = __uint_as_float(c_lo);
-      const bool stop = MAXHEAP ? (sv >= cv || cv < lose_below) : (sv <= cv);
-      const unsigned p_lo = stop ? s_lo : c_lo, p_hi = stop ? s_hi : c_hi;
-      if (act && !start_me) {
-        hp_sts_one(slot, p_lo, p_hi);
-        if (slot == root) outv[my_x + 1] = ((unsigned long long)p_hi << 32) | p_lo;
-        if (stop) { act = false; slot = capa; cur = capa; }
-        else {
-          slot = cur + (right ? 8u : 0u);
-          cur = min((slot << 1) - hb, capa);
-        }
-      }
-    }
-    // (4) the extraction that starts works on the root from the next tick on
-    if (start_me) { act = true; slot = root; cur = hb + 16u; }
-    __syncwarp();
-  }
-  ticks_out = ticks; stalls_out = stalls;
 }
 
 // ---- predicated stores / loads: a lane that has nothing to do skips the access without leaving the warp's common path
@@ -131,107 +48,22 @@ __device__ __forceinline__ void hp_lds_one_if(bool p, unsigned addr, unsigned &x
                : "+r"(x0), "+r"(x1) : "r"(addr), "r"((unsigned)p) : "memory");
 }
 
-// ---- the shipped loop.  The schedule of heap_extract_pipe_warp above, written for the issue slots of one warp:
+// ---- the loop, written for the issue slots of one warp:
 //   * no lane ever leaves the warp's common path: stores and the starting lane's accesses are predicated, every decision
 //     is a select (an `if (act) ...` region makes the warp diverge and reconverge in every tick: 257 vs 107 cycles/tick);
 //   * the extracted roots go to SHARED memory (`outs`, 8-byte entries; a global store in the tick costs ~40 cycles per
 //     extraction);
-//   * the start decision looks at the holes after the tick's move (fewer held-back starts when there is no loser cut);
 //   * both possible next pair addresses exist before the child comparison resolves and the stop test is one comparison,
 //     so the loop-carried chains are
 //     LDS.128 -> FSETP -> SEL -> VIMNMX -> LDS.128     (address)
 //     LDS.128 -> FMNMX -> FSETP -> SEL -> STS          (hole)
 // An idle lane sits on the sentinel pair `capa`; its "next pair" clamps back to capa by itself (2*capa - hb > capa).
-// FLAGS & 1 (micro-benchmark switch): no __syncwarp between ticks
-template <bool MAXHEAP, int FLAGS>
-__device__ __forceinline__ void heap_extract_pipe_warp4(unsigned long long *A, const int n, const int extract, const float lose_below,
-                                                        unsigned long long *outs, const int maxt, const unsigned lane,
-                                                        unsigned &ticks_out, unsigned &stalls_out) {
-  constexpr int NL = 16;
-  constexpr unsigned FULL = 0xffffffffu;
-  const unsigned hb = hp_smem_u32(A);
-  const unsigned ob = hp_smem_u32(outs);
-  const unsigned sent = MAXHEAP ? 0xff800000u : 0x7f800000u;
-  const unsigned capa = hb + (((unsigned)(maxt >> 1) + 1u) << 4);
-  const unsigned root = hb + 8u;
-  bool act = false;
-  unsigned slot = capa, cur = capa;
-  unsigned s_lo = sent, s_hi = 0u;
-  unsigned my_out = ob;                                    // where this lane's root write goes: outs[my_x + 1]
-  int next_x = 0;
-  unsigned ticks = 0, stalls = 0;
-  unsigned nxt_lo, nxt_hi;
-  hp_lds_one(hb + ((unsigned)n << 3), nxt_lo, nxt_hi);
-  if (lane == 0 && extract > 0) outs[0] = A[1];
-  // The stop test of a max-heap level, "s >= c || c < lose_below" (c = the larger child), is ONE comparison against
-  // thr = max(s, nextdown(lose_below)):  if s >= lose_below then c < lose_below implies c <= s, so the test is c <= s;
-  // otherwise c <= s implies c < lose_below, so the test is c < lose_below, i.e. c <= nextdown(lose_below).
-  // (Scores are finite or the -inf sentinel, never NaN.)  Min-heap: "s <= c" (c = the smaller child), no cut.
-  float lose_dn = lose_below;
-  if (MAXHEAP && lose_below > -INFINITY) {
-    unsigned b = __float_as_uint(lose_below);
-    b = (lose_below > 0.0f) ? b - 1u : (lose_below < 0.0f) ? b + 1u : 0x80000001u;
-    lose_dn = __uint_as_float(b);
-  }
-#define HP_STEP4()                                                                                                       \
-  {                                                                                                                      \
-    const unsigned base2 = (cur << 1) - hb;                                                                              \
-    const unsigned curL = min(base2, capa), curR = min(base2 + 16u, capa);                                               \
-    const float sv = __uint_as_float(s_lo), xv = __uint_as_float(x0), yv = __uint_as_float(y0);                          \
-    const float thr = MAXHEAP ? fmaxf(sv, lose_dn) : sv;                                                                 \
-    const bool right = MAXHEAP ? (xv < yv) : (xv > yv);                                                                  \
-    const float cv = MAXHEAP ? fmaxf(xv, yv) : fminf(xv, yv);                                                            \
-    const bool stop = MAXHEAP ? (cv <= thr) : (cv >= thr);                                                               \
-    const unsigned c_lo = right ? y0 : x0, c_hi = right ? y1 : x1;                                                       \
-    const unsigned p_lo = stop ? s_lo : c_lo, p_hi = stop ? s_hi : c_hi;                                                 \
-    hp_sts_one_if(act, slot, p_lo, p_hi);                                                                                \
-    hp_sts_one_if(act && slot == root, my_out, p_lo, p_hi);                                                              \
-    const bool go = act && !stop;                                                                                        \
-    slot = go ? cur + (right ? 8u : 0u) : capa;                                                                          \
-    cur = right ? curR : curL;                                                                                           \
-    act = go;                                                                                                            \
-  }
-  int wait = 0;
-  while (true) {
-    // ---- one tick: every extraction in flight fills its hole and moves one level down
-    unsigned x0, x1, y0, y1;
-    hp_lds_pair(cur, x0, x1, y0, y1);
-    HP_STEP4()
-    // ---- every second tick (or every tick while a start is held back): may the next extraction start?  Decided on
-    //      the holes as they are AFTER this tick's move; its first level is the next tick's business
-    if (--wait <= 0) {
-      if (next_x >= extract) {
-        if (!__any_sync(FULL, act)) break;
-      } else {
-        const unsigned ms = (unsigned)(n - next_x);
-        bool ok = true;
-        if (!(MAXHEAP && (__uint_as_float(nxt_lo) < lose_below))) {          // rare with the loser cut
-          const unsigned h = (slot - hb) >> 3;
-          const int dh = 31 - __clz(h), dms = 31 - __clz(ms);
-          ok = !__any_sync(FULL, act && dms >= dh && (ms >> (dms - dh)) == h);
-        }
-        if (ok) {
-          const bool start_me = (lane == ((unsigned)next_x & (NL - 1)));
-          const unsigned ma = hb + (ms << 3);
-          hp_lds_one_if(start_me, ma, s_lo, s_hi);                           // s = A[m]
-          hp_sts_one_if(start_me, ma, sent, 0u);                             // slot m leaves the heap
-          next_x++;
-          my_out = start_me ? ob + ((unsigned)next_x << 3) : my_out;         // outs[x + 1]
-          hp_lds_one(hb + ((unsigned)(n - next_x) << 3), nxt_lo, nxt_hi);
-          act = act || start_me;
-          slot = start_me ? root : slot;
-          cur = start_me ? hb + 16u : cur;
-          wait = 2;
-        } else stalls++;
-      }
-    }
-    if (!(FLAGS & 1)) __syncwarp();
-    ticks++;
-  }
-#undef HP_STEP4
-  ticks_out = ticks; stalls_out = stalls;
-}
-
+//
+// The stop test of a max-heap level, "s >= c || c < lose_below" (c = the larger child), is ONE comparison against
+// thr = max(s, nextdown(lose_below)):  if s >= lose_below then c < lose_below implies c <= s, so the test is c <= s;
+// otherwise c <= s implies c < lose_below, so the test is c < lose_below, i.e. c <= nextdown(lose_below).
+// (Scores are finite or the -inf sentinel, never NaN.)  Min-heap: "s <= c" (c = the smaller child), no cut.
+//
 // ---- the step in PTX.  One warp issues about one instruction every two cycles however little they depend on each other,
 // so once the shared-memory round trip is covered (~64 cycles with the compare and the address select: "tick floor" in
 // tools/ubench/heapx.cu) a tick costs its instruction count.  The step below is 24 instructions; the address arithmetic
@@ -294,11 +126,14 @@ __device__ __forceinline__ void hp_step(unsigned &cur, unsigned &slot, unsigned 
 #undef HP_STEP_TAIL
 }
 
-template <bool MAXHEAP, int FLAGS>
+// Called by the 32 threads of one warp (lane = 0..31).  A: heap entries (low word = fp32 score bits, high word = token
+// id), slot h = heap index h, sentinel padded; n: heap size; outs[k] = k-th extracted root, k = 0..extract (the last
+// entry is what would be extracted next).  Returns the number of ticks / held-back starts through the pointers.
+template <bool MAXHEAP>
 __device__ __forceinline__ void heap_extract_pipe_warp6(unsigned long long *A, const int n, const int extract, const float lose_below,
                                                         unsigned long long *outs, const int maxt, const unsigned lane,
                                                         unsigned &ticks_out, unsigned &stalls_out) {
-  constexpr int NL = 16;
+  constexpr int NL = 16;                                   // extraction x is owned by lane x mod NL
   constexpr unsigned FULL = 0xffffffffu;
   const unsigned hb = hp_smem_u32(A);
   const unsigned ob = hp_smem_u32(outs);
@@ -348,7 +183,7 @@ __device__ __forceinline__ void heap_extract_pipe_warp6(unsigned long long *A, c
         } else stalls++;
       }
     }
-    if (!(FLAGS & 1)) __syncwarp();
+    __syncwarp();
     ticks++;
   }
   ticks_out = ticks; stalls_out = stalls;

@@ -115,15 +115,6 @@ def test_fast_heap_replay_agrees_with_sequential_replay(monkeypatch):
             _check(r, u)
 
 
-def test_forced_sequential_heap_gives_same_trellis(monkeypatch):
-    monkeypatch.setenv("JB200_FORCE_SEQ_HEAP", "1")
-    g = Golden("small_b100")
-    am = capi.GmmScorer(g.ds, mode=capi.GMM_EXACT)
-    dec = capi.Decoder(g.ds, am, max_utts=8, max_frames=4096)
-    for r, u in zip(dec.decode(g.feats), g.utts):
-        _check(r, u)
-
-
 def test_grammar_mode_trellis_matches_reference():
     g = Golden("small_dfa")
     am = capi.GmmScorer(g.ds, mode=capi.GMM_EXACT)

@@ -45,34 +45,28 @@ def main():
     dev = [torch.from_numpy(b).cuda() for b in batches]
     print(f"# {name}: resident {resident}, inputs sampled in {time.time() - t0:.1f}s", flush=True)
     lib = capi.lib()
-    # (label, utterances, pipeline frames, environment)
+    # (label, utterances, pipeline frames)
     B3 = (resident * 3) // 4
     configs = [
-        ("base", resident, 0, {}),
-        ("host_numbering", resident, 0, {"JB200_NO_RENUMBER": "1"}),
-        ("no_relocate", resident, 0, {"JB200_NO_RELOCATE": "1"}),
-        ("b3_pipe32", B3, 32, {}),
-        ("b3_nopipe", B3, 0, {}),
-        ("b3_pipe250", B3, 250, {}),
-        ("b3_pipe125", B3, 125, {}),
-        ("b3_pipe64", B3, 64, {}),
-        ("b4_pipe125", resident, 125, {}),
+        ("base", resident, 0),
+        ("b3_pipe32", B3, 32),
+        ("b3_nopipe", B3, 0),
+        ("b3_pipe250", B3, 250),
+        ("b3_pipe125", B3, 125),
+        ("b3_pipe64", B3, 64),
+        ("b4_pipe125", resident, 125),
     ]
     if len(sys.argv) > 3:
         # either names of the presets above, or explicit label:utterances:pipe_frames triples
         sel = sys.argv[3].split(",")
         if all(":" in x for x in sel):
-            configs = [(x.split(":")[0], int(x.split(":")[1]), int(x.split(":")[2]), {}) for x in sel]
+            configs = [(x.split(":")[0], int(x.split(":")[1]), int(x.split(":")[2])) for x in sel]
         else:
             configs = [c for c in configs if c[0] in set(sel)]
     B3 = min(c[1] for c in configs)
     fps = {}
-    for label, B, pipe, env in configs:
-        for k, v in env.items():
-            os.environ[k] = v
+    for label, B, pipe in configs:
         dec = capi.Decoder(ds, am, max_utts=B, max_frames=B * T)
-        for k in env:
-            del os.environ[k]
         dec.set_pipeline(pipe)
         off = (np.arange(B + 1, dtype=np.int32) * T)
         offp = off.ctypes.data_as(C.POINTER(C.c_int32))

@@ -31,8 +31,7 @@ __device__ __forceinline__ unsigned heap_pick(unsigned x0, unsigned y0, unsigned
   return r;
 }
 
-// V: 9 = the pipelined warp replay of heap_pipe.cuh, readable form; 14 = lock-step form in C++ (15: without __syncwarp);
-// 18 = the shipped form, step in PTX (19: without __syncwarp);
+// V: 18 = the pipelined warp replay of heap_pipe.cuh (what beam.cu ships);
 // single-thread variants: 0 = round 1's loop; 1 = outv in shared memory; 2 = no loser-cut test; 3 = non-volatile (sinkable) load;
 //    4 = one level per loop trip (no ping-pong unroll); 5 = plain load whose result is also consumed on the
 //    exit path (ptxas must issue it ahead of the stop test); 6 = 5 + both grandchild pairs requested one level
@@ -243,21 +242,16 @@ __global__ void __launch_bounds__(256, 4) k(const unsigned long long *init, int 
   for (int i = threadIdx.x; i < MAXT + 4; i += blockDim.x) A[i] = (i >= 1 && i <= n) ? init[i] : 0xff800000ull;
   __syncthreads();
   int extract = extract_in;
-  if (V >= 9) {
-    // variant 9: the pipelined warp replay of heap_pipe.cuh (what beam.cu ships)
+  if (V == 18) {
     if (threadIdx.x < 32) {
       unsigned ticks, stalls;
       long long t0 = clock64();
-      if (V == 9) jb200::heap_extract_pipe_warp<true>(A, n, extract, lose_below, outg + (size_t)blockIdx.x * 1024, MAXT, threadIdx.x, ticks, stalls);
-      else if (V == 14) jb200::heap_extract_pipe_warp4<true, 0>(A, n, extract, lose_below, outs, MAXT, threadIdx.x, ticks, stalls);
-      else if (V == 15) jb200::heap_extract_pipe_warp4<true, 1>(A, n, extract, lose_below, outs, MAXT, threadIdx.x, ticks, stalls);
-      else if (V == 18) jb200::heap_extract_pipe_warp6<true, 0>(A, n, extract, lose_below, outs, MAXT, threadIdx.x, ticks, stalls);
-      else jb200::heap_extract_pipe_warp6<true, 1>(A, n, extract, lose_below, outs, MAXT, threadIdx.x, ticks, stalls);
+      jb200::heap_extract_pipe_warp6<true>(A, n, extract, lose_below, outs, MAXT, threadIdx.x, ticks, stalls);
       long long t1 = clock64();
       if (threadIdx.x == 0) { res[blockIdx.x * 2] = t1 - t0; res[blockIdx.x * 2 + 1] = ticks; }
     }
     __syncthreads();
-    if (V >= 14) for (int i = threadIdx.x; i < extract_in; i += blockDim.x) outg[(size_t)blockIdx.x * 1024 + i] = outs[i];
+    for (int i = threadIdx.x; i < extract_in; i += blockDim.x) outg[(size_t)blockIdx.x * 1024 + i] = outs[i];
     return;
   }
   if (threadIdx.x == 0) {
@@ -320,7 +314,7 @@ __global__ void __launch_bounds__(256, 4) kfloor(const unsigned long long *init,
     long long t0 = clock64();
     for (int t = 0; t < nticks; t++) {
       unsigned x0, x1, y0, y1;
-      jb200::hp_lds_pair(cur, x0, x1, y0, y1);
+      lds_pair(cur, x0, x1, y0, y1);
       const bool right = __uint_as_float(x0) < __uint_as_float(y0);
       const unsigned base2 = (cur << 1) - hb;
       unsigned ncur = min(base2 + (right ? 16u : 0u), capa);
@@ -377,7 +371,7 @@ int main() {
     printf("blocks %3d tick floor mode %d: %.1f cycles/tick\n", blocks, mode, sfl / blocks / nt);
   }
   for (int blocks : {1, WAVE}) {
-    for (int v : {5, 14, 18, 19}) {
+    for (int v : {5, 18}) {
       for (int rep = 0; rep < 2; rep++) {
         switch (v) {
           case 0: k<0><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
@@ -389,11 +383,7 @@ int main() {
           case 6: k<6><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
           case 7: k<7><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
           case 8: k<8><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
-          case 9: k<9><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
-          case 14: k<14><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
-          case 15: k<15><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
           case 18: k<18><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
-          case 19: k<19><<<blocks, 256>>>(d, n, extract, lose_below, o, r); break;
         }
         cudaDeviceSynchronize();
       }
