@@ -159,6 +159,10 @@ int jb200_decoder_heap_stats(jb200_decoder *d, int64_t out[3]);
 int jb200_decoder_select_stats(jb200_decoder *d, int64_t out[2]);
 /* of the closed-form answers, how many needed the exact treatment of re-inserted elements (closed form with relocations) */
 int64_t jb200_decoder_relocated_selects(jb200_decoder *d);
+/* where the beam cut's heap-select array lives: out[0] 1 in global memory (token sets too large for shared memory),
+ * 0 in shared memory; and, since create, how many replays of a global-memory heap ran on a shared-memory copy of the
+ * whole heap (out[1]) and on the heap itself with its top levels and tail copied into shared memory (out[2]) */
+int jb200_decoder_cut_placement(jb200_decoder *d, int64_t out[3]);
 /* how many utterances (thread blocks) are co-resident on the device for this decoder */
 int jb200_decoder_resident_utts(const jb200_decoder *d);
 /* SM-cycle totals per kernel phase of the first n_utts utterances of the last batch: cycles [n_utts][8]

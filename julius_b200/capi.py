@@ -74,6 +74,7 @@ def lib():
             L.jb200_decoder_select_stats.argtypes = [vp, C.POINTER(C.c_int64)]
             L.jb200_decoder_relocated_selects.argtypes = [vp]
             L.jb200_decoder_relocated_selects.restype = C.c_int64
+            L.jb200_decoder_cut_placement.argtypes = [vp, C.POINTER(C.c_int64)]
             L.jb200_decoder_phase_cycles.argtypes = [vp, C.POINTER(C.c_int64), C.c_int]
             U8 = C.POINTER(C.c_uint8)
             L.jb200_decoder_set_pipeline.argtypes = [vp, C.c_int]
@@ -327,6 +328,12 @@ class Decoder:
         return {"fallbacks": int(v[0]), "levels": int(v[1]), "extractions": int(v[2]),
                 "upward_selects": int(w[0]), "closed_form": int(w[1]),
                 "closed_form_relocated": int(lib().jb200_decoder_relocated_selects(self._h))}
+
+    def cut_placement(self) -> dict:
+        """where the heap-select array lives, and the replays of a global-memory heap since create by copy strategy"""
+        v = (C.c_int64 * 3)()
+        _check(lib().jb200_decoder_cut_placement(self._h, v), "jb200_decoder_cut_placement")
+        return {"heap_global": bool(v[0]), "whole_copy_replays": int(v[1]), "top_tail_replays": int(v[2])}
 
     def resident_utts(self) -> int:
         return int(lib().jb200_decoder_resident_utts(self._h))

@@ -130,6 +130,7 @@ struct BeamParams {
   // chunked launches
   const ChunkDesc *chunk; UttState *state; int interim; int *interim_words;   // [n_utts][MAX_WORDS]
   int atoms_in_place;       // streams: the finalized atoms of utterance u go to atoms_out + atom_off[u] (no batch compaction)
+  unsigned long long *heap_chk;   // JB200_CHECK_HEAP on a multipath tree: [n_utts][maxt+4] input of the sequential replay
 };
 
 // ---- small device helpers ----------------------------------------------------------------------
@@ -538,7 +539,7 @@ __device__ void heap_extract_fast(const CutAreas &ca, const int n, const int ext
       heap_extract_pipe_warp6<MAXHEAP>(gcache, n, extract, lose_below, outv, lmaxt, threadIdx.x, ticks, stalls);
       if (threadIdx.x == 0) {
         atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
-        atomicAdd(stats + 3, (unsigned long long)stalls);
+        atomicAdd(stats + 3, (unsigned long long)stalls); atomicAdd(stats + 7, 1ull);
       }
     }
     __syncthreads();
@@ -565,6 +566,7 @@ __device__ void heap_extract_fast(const CutAreas &ca, const int n, const int ext
     if (threadIdx.x == 0) {
       atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
       atomicAdd(stats + 3, (unsigned long long)stalls);
+      if (!__isShared(A)) atomicAdd(stats + 8, 1ull);
     }
   }
   __syncthreads();
@@ -1129,8 +1131,39 @@ __device__ __forceinline__ int select_exact(const CutAreas &ca, int n, int need,
   return start;
 }
 
+// Self-check of a multipath select (JB200_CHECK_HEAP): the plain sequential select (heap_build + heap_extract_seq) of the
+// select's input chk[1..n], compared with what the kernel made -- the whole arrangement heap[1..n] (select #1: select #2
+// starts from it), or, with heap == nullptr, the survivors in visiting order ordn[0..need) (select #2).  Overflow code 4
+// on a difference.  With tok != nullptr the input is first rebuilt from the tokens in creation order (select #1).  With
+// overflow == nullptr it only copies heap[1..n] to chk (the input of select #2, which the cut destroys).  All threads
+// call it.
+__device__ __noinline__ void check_select_mp(unsigned long long *chk, const int n, const int need, const Tok *tok,
+                                             const unsigned long long *heap, const int *ordn, int *overflow) {
+  if (!overflow) {
+    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) chk[h] = heap[h];
+    __syncthreads();
+    return;
+  }
+  const bool upward = (need < n - need);
+  if (tok) for (int r = threadIdx.x; r < n; r += BEAM_THREADS) chk[r + 1] = ((unsigned long long)(unsigned)r << 32) | __float_as_uint(tok[r].score);
+  __syncthreads();
+  if (upward) { heap_build<true>(chk, n); heap_extract_seq<true>(chk, n, need); }
+  else { heap_build<false>(chk, n); heap_extract_seq<false>(chk, n, n - need); }
+  bool bad = false;
+  if (heap) {
+    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) bad |= (chk[h] != heap[h]);
+  } else {
+    const int start = upward ? n - need : 0;
+    for (int k = threadIdx.x; k < need; k += BEAM_THREADS) bad |= (ordn[k] != (int)(chk[start + k + 1] >> 32));
+  }
+  if (bad) *overflow = 4;
+  __syncthreads();
+}
+
 static constexpr int TOK_EXISTS = 0x40000000;
 
+// CHECK: the JB200_CHECK_HEAP build of the kernel (the self-check stays out of the shipped kernel's register budget)
+template <bool CHECK>
 __global__ void __launch_bounds__(BEAM_THREADS, BEAM_MINBLOCKS)
 beam_kernel_mp(const BeamParams p) {
   const int u = blockIdx.x;
@@ -1341,6 +1374,7 @@ beam_kernel_mp(const BeamParams p) {
         ns_a = need;
         if (need < ncre_a - need) select_exact<true>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
         else select_exact<false>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
+        if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre_a, need, tn, heap, nullptr, &s_overflow);
       }
     }
     __syncthreads();
@@ -1392,7 +1426,8 @@ beam_kernel_mp(const BeamParams p) {
       }
       if (tid == 0) { s_natoms = min(carry_a, atom_cap); s_E = min(carry_w, MAXW); }
       nbits_b = carry_w * p.n_isoarc + p.n_sharc;
-      if (carry_w > MAXW || nbits_b > p.maxbits) { if (tid == 0) s_overflow = 1; nbits_b = 0; }
+      // carry_a > atom_cap: some word ends got no atom and no wend entry, and wend[0..E) would hold stale entries
+      if (carry_w > MAXW || nbits_b > p.maxbits || carry_a > atom_cap) { if (tid == 0) s_overflow = 1; nbits_b = 0; }
     }
     if (final) { n_left = ncre_a; __syncthreads(); break; }
     nwords = (nbits_b + 31) >> 5;
@@ -1566,8 +1601,11 @@ beam_kernel_mp(const BeamParams p) {
       // tindex order = select #1's arrangement, then the new tokens
       for (int k = tid; k < ns_new; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
     } else {
+      // the input of select #2 cannot be rebuilt after the cut: the self-check keeps a copy
+      if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre, 0, nullptr, heap, nullptr, nullptr);
       beam_cut(p, ca, ncre, s_hmaxkey, tn, slots, ordn, s_prof, s_tprev);
       slots_clean = true;
+      if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre, p.beam, nullptr, nullptr, ordn, &s_overflow);
     }
     PROF_MARK(6);
     if (tid == 0) {
@@ -1959,10 +1997,13 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.bitmask));
   TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.wordpre));
   // beam-cut counters: [0] fall-backs to the plain sequential replay (there are none: always 0), [1] replay ticks,
-  // [2] extractions replayed, [3] held-back starts, [4] upward selects, [5] of which closed form, [6] of which with relocations
-  TRY(dev_alloc(d, 8, &P.misspec_counter));
-  TRYC(cudaMemset(P.misspec_counter, 0, 8 * sizeof(unsigned long long)));
+  // [2] extractions replayed, [3] held-back starts, [4] upward selects, [5] of which closed form, [6] of which with relocations,
+  // global-memory heap only: [7] replays on a shared-memory copy of the whole heap, [8] replays on the heap itself (top-and-tail copy)
+  TRY(dev_alloc(d, 16, &P.misspec_counter));
+  TRYC(cudaMemset(P.misspec_counter, 0, 16 * sizeof(unsigned long long)));
   P.check_heap = getenv("JB200_CHECK_HEAP") ? atoi(getenv("JB200_CHECK_HEAP")) : 0;
+  P.heap_chk = nullptr;
+  if (P.check_heap && P.multipath) TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_chk));
   P.lmc_bits = lmc_bits; P.lmc = nullptr;
   if (lmc_bits > 0) {
     TRY(dev_alloc_shared(d, (size_t)1 << lmc_bits, &P.lmc));
@@ -2016,7 +2057,7 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   }
   d->smem_bytes = (heap_global ? (size_t)P.qcap * 8 + (size_t)(t->beam_width + 2) * 8 : (size_t)(maxt + 4) * 8) + offs_bytes;
   d->grammar = grammar;
-  const void *kern = grammar ? (const void *)beam_kernel_grammar : P.multipath ? (const void *)beam_kernel_mp : (const void *)beam_kernel;
+  const void *kern = grammar ? (const void *)beam_kernel_grammar : P.multipath ? (P.check_heap ? (const void *)beam_kernel_mp<true> : (const void *)beam_kernel_mp<false>) : (const void *)beam_kernel;
   TRYC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
   {
     int per_sm = 0, sms = 0;
@@ -2108,7 +2149,8 @@ static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index = 0, int in
   P.chunk = d->d_chunk + (size_t)chunk_index * d->max_utts; P.state = d->d_state;
   P.interim = interim; P.interim_words = d->d_interim_words; P.atoms_in_place = d->stream_mode ? 1 : 0;
   if (d->grammar) beam_kernel_grammar<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
-  else if (P.multipath) beam_kernel_mp<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
+  else if (P.multipath && P.check_heap) beam_kernel_mp<true><<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
+  else if (P.multipath) beam_kernel_mp<false><<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
   else beam_kernel<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
   JB_LAUNCH_CHECK();
   return JB200_OK;
@@ -2239,6 +2281,15 @@ extern "C" int64_t jb200_decoder_relocated_selects(jb200_decoder *d) {
   cudaSetDevice(d->device);
   if (cudaMemcpy(&v, d->P.misspec_counter + 6, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   return (int64_t)v;
+}
+
+extern "C" int jb200_decoder_cut_placement(jb200_decoder *d, int64_t out[3]) {
+  if (!d || !out) { set_error("bad argument"); return JB200_ERR_ARG; }
+  unsigned long long v[2] = {0, 0};
+  JB_CUDA(cudaSetDevice(d->device));
+  JB_CUDA(cudaMemcpy(v, d->P.misspec_counter + 7, sizeof(v), cudaMemcpyDeviceToHost));
+  out[0] = d->P.heap_g ? 1 : 0; out[1] = (int64_t)v[0]; out[2] = (int64_t)v[1];
+  return JB200_OK;
 }
 
 extern "C" int64_t jb200_decoder_last_d2h_bytes(const jb200_decoder *d) { return d ? d->last_d2h : 0; }

@@ -12,6 +12,10 @@ Each fixture directory holds
     python tests/golden/make_golden.py sweep
 
 writes the option sweeps of tests/test_oracle_sweep.py as sweep/<case>.npz, in a compact form (tests/util.py).
+
+    python tests/golden/make_golden.py sweep --missing
+
+writes only the sweep cases that have no file yet and leaves the existing ones untouched.
 """
 import json
 import os
@@ -64,11 +68,13 @@ DNN_CASES = {
 }
 
 
-def make_sweep():
+def make_sweep(missing_only=False):
     from test_oracle_sweep import SWEEP, GRAMMAR_SWEEP
     cases = [(p, e, False, dict(n_utts=2, n_frames=150, noise_utts=1)) for p, e in SWEEP]
     cases += [("small", e, True, dict(n_utts=2, n_frames=180, noise_utts=1)) for e in GRAMMAR_SWEEP]
     for preset, extra, grammar, kw in cases:
+        if missing_only and os.path.exists(os.path.join(util.SWEEP_DIR, util.sweep_name(preset, extra, grammar) + ".npz")):
+            continue
         tmp = tempfile.mkdtemp(prefix="jb200_golden_")
         m, files, dump, out = fixtures.make_fixture(preset, tmp, extra_args=extra, grammar=grammar, **kw)
         blob = refdump.load_blob(os.path.join(tmp, "model.jb2m"))
@@ -80,8 +86,8 @@ def make_sweep():
 
 def main():
     ffi.build()
-    if sys.argv[1:] == ["sweep"]:
-        return make_sweep()
+    if sys.argv[1:2] == ["sweep"]:
+        return make_sweep(missing_only=sys.argv[2:] == ["--missing"])
     only = set(sys.argv[1:])
     for name, (preset, nu, nf, nn, extra) in CASES.items():
         if only and name not in only:

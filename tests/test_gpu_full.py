@@ -152,6 +152,57 @@ def test_wide_beam_4000_vs_oracle(name, oracle_lib):
     assert max(c[1] for c in o["trace"]) > 800      # the wide beam was actually used
 
 
+@pytest.mark.parametrize("name", ["tri20k", "tri20k_mp"])
+def test_wide_beam_4000_heap_self_check(name, monkeypatch, oracle_lib):
+    """The inputs of test_wide_beam_4000_vs_oracle with JB200_CHECK_HEAP=1: every cut of the global-memory heap,
+    upward ones included, against the plain sequential heap select (both selects of a multipath frame)."""
+    if not workload.ready(name):
+        pytest.skip(f"workloads/{name} not prepared")
+    monkeypatch.setenv("JB200_CHECK_HEAP", "1")
+    ds = desc.Descriptors(workload.load_model(name))
+    ds.tree.beam_width = 4000
+    m = workload.synth_model(name)
+    am = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
+    dec = capi.Decoder(ds, am, max_utts=2, max_frames=2 * 120)
+    feats = workload.sample_batch(m, 2, 120, seed=91)
+    for x, r in zip(feats, dec.decode(feats)):
+        o = oracle_lib.beam_decode(ds, oracle_lib.gmm_score(ds, x))
+        assert r["overflow"] == 0
+        ok, why = atoms_equal(r["atoms"], o["atoms"])
+        assert ok, why
+    pl, hs = dec.cut_placement(), dec.heap_stats()
+    print(name, pl, hs)
+    assert pl["heap_global"]
+    assert hs["upward_selects"] > 0
+    # the multipath tree creates frames of more than qcap (16384) tokens, which are replayed on the global heap itself
+    # (top-and-tail copy); the normal tree stays below that and every replay runs on the whole-heap copy
+    assert (pl["top_tail_replays"] if name == "tri20k_mp" else pl["whole_copy_replays"]) > 0
+
+
+def test_dnn60k_mp_heap_self_check(monkeypatch, oracle_lib):
+    """The inputs of test_dnn_hmm_configs_vs_oracle[dnn60k_mp] on the restatement's scores with JB200_CHECK_HEAP=1.
+    Frames of more than qcap (16384) tokens do not fit the shared-memory copy of the global heap and are replayed on
+    the heap itself with its top levels and tail copied (heap_extract_pipe_global): the counter shows it ran."""
+    name, frames = "dnn60k_mp", 150
+    if not workload.ready(name):
+        pytest.skip(f"workloads/{name} not prepared")
+    monkeypatch.setenv("JB200_CHECK_HEAP", "1")
+    ds = desc.Descriptors(workload.load_model(name))
+    m = workload.synth_model(name)
+    feats = workload.sample_inputs(name, m, 2, frames, seed=61)
+    am = capi.GmmScorer(ds, gmm_desc=ds.cd_only_gmm())
+    dec = capi.Decoder(ds, am, max_utts=2, max_frames=2 * frames)
+    scores = [oracle_lib.dnn_score(ds, x) for x in feats]
+    for r, sc in zip(dec.decode_scores(scores), scores):
+        o = oracle_lib.beam_decode(ds, sc)
+        assert r["overflow"] == 0
+        ok, why = atoms_equal(r["atoms"], o["atoms"])
+        assert ok, why
+    pl = dec.cut_placement()
+    print(name, pl, dec.heap_stats())
+    assert pl["heap_global"] and pl["top_tail_replays"] > 0
+
+
 @pytest.mark.parametrize("name,frames", [("dnn20k", 200), ("dnn60k_mp", 150)])
 def test_dnn_hmm_configs_vs_oracle(name, frames, oracle_lib):
     """BASELINE.json configs[3] (DNN-HMM 528 -> 7 x 2048 -> 3000 states, 20k words) and configs[4] (the same acoustic

@@ -13,6 +13,13 @@ from test_oracle_sweep import SWEEP, GRAMMAR_SWEEP
 pytestmark = pytest.mark.gpu
 
 
+def _room_for_atoms(monkeypatch, feats, utts):
+    """the decoder keeps room for 64 trellis words a frame on average; the widest sweep cases (-b 2500) store more"""
+    need = max(-(-len(u.atoms) // len(x)) + 1 for u, x in zip(utts, feats))
+    if need > 64:
+        monkeypatch.setenv("JB200_ATOMS_PER_FRAME", str(need))
+
+
 def _check(r, u):
     ok, why = atoms_equal(r["atoms"], u.atoms)
     assert ok, why
@@ -21,8 +28,9 @@ def _check(r, u):
 
 
 @pytest.mark.parametrize("preset,extra", SWEEP, ids=[" ".join([p] + e) for p, e in SWEEP])
-def test_gpu_path_equals_compiled_reference(preset, extra):
+def test_gpu_path_equals_compiled_reference(preset, extra, monkeypatch):
     ds, feats, utts = load_sweep_case(preset, extra)
+    _room_for_atoms(monkeypatch, feats, utts)
     am = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
     for u, x in zip(utts, feats):
         assert scores_sha(am.score(x)) == u.outprob_sha256, "state scores differ from the reference"
@@ -33,8 +41,9 @@ def test_gpu_path_equals_compiled_reference(preset, extra):
 
 # the GPU beam takes grammars on normal trees only (creation refuses -multipath loudly, tested in test_gpu_beam.py)
 @pytest.mark.parametrize("extra", [e for e in GRAMMAR_SWEEP if "-multipath" not in e], ids=lambda e: " ".join(e))
-def test_gpu_grammar_mode_equals_compiled_reference(extra):
+def test_gpu_grammar_mode_equals_compiled_reference(extra, monkeypatch):
     ds, feats, utts = load_sweep_case("small", extra, grammar=True)
+    _room_for_atoms(monkeypatch, feats, utts)
     am = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
     dec = capi.Decoder(ds, am, max_utts=4, max_frames=2048)
     for r, u in zip(dec.decode(feats), utts):

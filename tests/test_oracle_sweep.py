@@ -22,9 +22,15 @@ SWEEP = [
     ("small_tm", ["-gprune", "none", "-b", "100"]),              # tied-mixture codebooks, calc_tied_mix.c:161-248
     ("small_tm", ["-gprune", "safe", "-tmix", "2", "-b", "80", "-multipath"]),
 ]
+# beam widths at the edges of the beam cut (tests/test_gpu_beam_widths.py decodes the golden cases at the same widths
+# against the restatement): a search that finds no sentence end (-b 2), fewer than 16 extractions in flight and a small histogram
+# (-b 17), upward and downward cuts mixed (-b 300), only downward cuts and, on the device, the heap in global memory (-b 2500)
+WIDTHS = ["2", "17", "300", "2500"]
+SWEEP += [("small", ["-b", b]) for b in WIDTHS] + [("small", ["-multipath", "-b", b]) for b in WIDTHS]
 
 
 GRAMMAR_SWEEP = [["-b", "100"], ["-b", "60", "-penalty1", "-2.5", "-iwcd1", "max"], ["-b", "150", "-multipath", "-penalty1", "1.5"]]
+GRAMMAR_SWEEP += [["-b", b] for b in WIDTHS]
 
 
 @pytest.mark.parametrize("extra", GRAMMAR_SWEEP, ids=[" ".join(e) for e in GRAMMAR_SWEEP])
