@@ -1,10 +1,19 @@
-// common.cu -- error string, launch counter, version.
+// common.cu -- error string, launch counter, version, addlog table.
 #include "common.cuh"
 #include <cstdarg>
+#include <cmath>
 
 namespace jb200 {
 static thread_local char g_err[1024] = "";
 std::atomic<int64_t> g_launches{0};
+
+void build_addlog_table(std::vector<float> &tbl) {
+  tbl.resize(ADDLOG_TABLE_N);
+  for (int i = 0; i < ADDLOG_TABLE_N; i++) {
+    float f = -((float)15 * (float)i / (float)ADDLOG_TABLE_N);
+    tbl[i] = (float)log(1 + exp((double)f));
+  }
+}
 
 void set_error(const char *fmt, ...) {
   va_list ap;

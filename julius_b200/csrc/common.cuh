@@ -6,12 +6,27 @@
 #include <cstring>
 #include <string>
 #include <atomic>
+#include <vector>
 #include "julius_b200.h"
 
 namespace jb200 {
 
 void set_error(const char *fmt, ...);
 extern std::atomic<int64_t> g_launches;
+
+// ---- addlog_array (addlog.c:28-57,102-123): table-driven log-add, used by K1 and K2 ---------------
+static constexpr int ADDLOG_TABLE_N = 500000;
+// the 500 000-entry log(1 + exp(-x)) table, built with the same libm calls as addlog.c:39-57
+void build_addlog_table(std::vector<float> &tbl);
+// one step of the walk, addlog.c:112-120: y is the running sum, x the next term.  The drop test compares the float
+// difference with the double LOG_ADDMIN; against LOG_ADDMIN rounded up to a float it is the same test.
+__device__ __forceinline__ float addlog_step_exact(float y, float x, const float *__restrict__ tbl) {
+  if (x > y) { float t = x; x = y; y = t; }
+  float tmp = __fsub_rn(x, y);
+  if (tmp < __double2float_ru(JB200_LOG_ADDMIN)) return y;
+  unsigned int idx = (unsigned int)__dadd_rn(__dmul_rn((double)(-tmp), 33333.3333), 0.5);
+  return __fadd_rn(y, __ldg(tbl + idx));
+}
 
 #define JB_CUDA(expr)                                                              \
   do {                                                                             \

@@ -3,7 +3,7 @@
 // Stands in for dnn_calc_outprob (libsent/src/phmm/calc_dnn.c:774-868): per frame a stack of
 //   dst = W.src + b   (calc_dnn_fma.c:18-95 / sub1 calc_dnn.c:509-523)
 //   hidden: logistic through a 320001-entry table with clamps (calc_dnn.c:342-369)
-//   output: linear, then log-softmax via addlog_array and "- log10 prior" (calc_dnn.c:862-865)
+//   output: linear, then log-softmax through addlog_array and "- log10 prior" (calc_dnn.c:862-865)
 // The reference does this one frame at a time (a GEMV stack, 130 MB of weights per frame); here
 // all frames of the batch go through one GEMM per layer:  C[frames x out] = A[frames x in] . W^T.
 //
@@ -22,8 +22,8 @@
 // wait for the next stage, and then run the epilogue from registers: bias, the reference's clamped
 // table logistic, and the next layer's operands already split into bf16 hi/lo.  The producer runs
 // ahead into the next tile meanwhile.  The last layer's epilogue writes fp32 logits; a row kernel then
-// does the log-softmax (with the reference's "drop terms more than 13.8 below the sum" rule) and
-// subtracts the log10 prior.
+// normalises them with a bit-exact replay of addlog_array (the reference's table-driven walk from the last
+// output to the first) and subtracts the log10 prior.
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -206,46 +206,40 @@ __global__ void split_bf16_kernel(const float *__restrict__ src, int M, int K, _
   lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
 }
 
-// log-softmax + prior, one block per frame (calc_dnn.c:862-865 with addlog_array's drop rule:
-// terms more than LOG_ADDMIN below the sum do not contribute, addlog.c:116)
-__global__ void __launch_bounds__(256)
-dnn_softmax_kernel(const float *__restrict__ logits, int ld_logits, int N, const float *__restrict__ prior,
-                   float *__restrict__ rows, int row_stride) {
-  __shared__ float s_red[8];
-  __shared__ float s_val;
-  const int t = blockIdx.x, tid = threadIdx.x;
-  const float *x = logits + (size_t)t * ld_logits;
-  auto block_max = [&](float v) {
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    if ((tid & 31) == 0) s_red[tid >> 5] = v;
-    __syncthreads();
-    if (tid < 32) { float w = (tid < 8) ? s_red[tid] : -INFINITY; for (int o = 4; o > 0; o >>= 1) w = fmaxf(w, __shfl_xor_sync(0xffffffffu, w, o)); if (tid == 0) s_val = w; }
-    __syncthreads();
-    const float r = s_val; __syncthreads(); return r;
-  };
-  auto block_sum = [&](float v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((tid & 31) == 0) s_red[tid >> 5] = v;
-    __syncthreads();
-    if (tid < 32) { float w = (tid < 8) ? s_red[tid] : 0.0f; for (int o = 4; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o); if (tid == 0) s_val = w; }
-    __syncthreads();
-    const float r = s_val; __syncthreads(); return r;
-  };
-  float mx = -INFINITY;
-  for (int i = tid; i < N; i += 256) mx = fmaxf(mx, x[i]);
-  mx = block_max(mx);
-  float s = 0.0f;
-  for (int i = tid; i < N; i += 256) s += expf(x[i] - mx);
-  s = block_sum(s);
-  const float lse1 = mx + logf(s);
-  const float cut = lse1 + (float)JB200_LOG_ADDMIN;
-  float s2 = 0.0f;
-  for (int i = tid; i < N; i += 256) { const float v = x[i]; if (v >= cut) s2 += expf(v - mx); }
-  s2 = block_sum(s2);
-  const float lse = mx + logf(s2);
-  float *out = rows + (size_t)t * row_stride;
-  for (int i = tid; i < N; i += 256)
-    out[i] = (float)(JB200_INV_LOG_TEN * (double)(x[i] - lse) - (double)__ldg(prior + i));
+// log-softmax + prior (calc_dnn.c:862-865).  The normaliser is addlog_array (addlog.c:102-123) replayed bit for bit:
+// the outputs are walked from N-1 down to 0 into a running fp32 sum y (start LOG_ZERO), a term more than LOG_ADDMIN
+// below y as it stands at that point of the walk is dropped, the others are added through the 500 000-entry table.
+// That walk is a chain of dependent table loads, so each lane runs the chain of its own frame (a warp takes 32 frames);
+// the warp stages 32 outputs of its 32 frames at a time through shared memory, read coalesced and transposed.  Then
+// the warp writes each of its frames' score rows together.
+static constexpr int SOFTMAX_WARPS = 4;
+__global__ void __launch_bounds__(32 * SOFTMAX_WARPS)
+dnn_softmax_kernel(const float *__restrict__ logits, int ld_logits, int N, int T, const float *__restrict__ prior,
+                   const float *__restrict__ addlog_tbl, float *__restrict__ rows, int row_stride) {
+  __shared__ float s_tile[SOFTMAX_WARPS][32][33];
+  const int lane = threadIdx.x & 31;
+  const int f0 = (blockIdx.x * SOFTMAX_WARPS + (threadIdx.x >> 5)) * 32;   // first frame of this warp
+  if (f0 >= T) return;
+  const int nf = min(32, T - f0);
+  float (*tile)[33] = s_tile[threadIdx.x >> 5];
+  float y = JB200_LOG_ZERO;
+  for (int hi = N - 1; hi >= 0; hi -= 32) {
+    // tile[r][c] = output hi - c of frame f0 + r: c is the position in the walk
+    const int i = hi - lane;
+    for (int r = 0; r < nf; r++) tile[r][lane] = (i >= 0) ? __ldg(logits + (size_t)(f0 + r) * ld_logits + i) : 0.0f;
+    __syncwarp();
+    const int cnt = min(32, hi + 1);
+    if (lane < nf)
+      for (int c = 0; c < cnt; c++) y = addlog_step_exact(y, tile[lane][c], addlog_tbl);
+    __syncwarp();
+  }
+  for (int r = 0; r < nf; r++) {
+    const float lp = __shfl_sync(0xffffffffu, y, r);
+    const float *x = logits + (size_t)(f0 + r) * ld_logits;
+    float *out = rows + (size_t)(f0 + r) * row_stride;
+    for (int i = lane; i < N; i += 32)
+      out[i] = (float)__dsub_rn(__dmul_rn(JB200_INV_LOG_TEN, (double)__fsub_rn(__ldg(x + i), lp)), (double)__ldg(prior + i));
+  }
 }
 
 }  // namespace jb200
@@ -267,7 +261,7 @@ struct DnnLayerDev {
 struct jb200_dnn {
   int device = 0, n_layers = 0, in_dim = 0, out_dim = 0, row_stride = 0;
   std::vector<DnnLayerDev> L;
-  float *d_prior = nullptr, *d_logistic = nullptr;
+  float *d_prior = nullptr, *d_logistic = nullptr, *d_addlog = nullptr;
   PFN_encodeTiled encode = nullptr;
   cudaStream_t stream = nullptr;
   // batch buffers
@@ -292,7 +286,7 @@ extern "C" void jb200_dnn_destroy(jb200_dnn *h) {
   if (!h) return;
   cudaSetDevice(h->device);
   for (auto &l : h->L) { cudaFree(l.w_hi); cudaFree(l.w_lo); cudaFree(l.bias); }
-  cudaFree(h->d_prior); cudaFree(h->d_logistic); cudaFree(h->d_in); cudaFree(h->d_logits); cudaFree(h->d_rows);
+  cudaFree(h->d_prior); cudaFree(h->d_logistic); cudaFree(h->d_addlog); cudaFree(h->d_in); cudaFree(h->d_logits); cudaFree(h->d_rows);
   for (int i = 0; i < 2; i++) { cudaFree(h->act_hi[i]); cudaFree(h->act_lo[i]); }
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
@@ -300,6 +294,14 @@ extern "C" void jb200_dnn_destroy(jb200_dnn *h) {
 
 extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn **out) {
   if (!d || !out || d->n_layers < 1 || d->n_layers > JB200_DNN_MAX_LAYERS) { set_error("jb200_dnn_create: bad argument"); return JB200_ERR_ARG; }
+  // the kernels trust these: the input copy is in_dim wide, the last layer writes layer_out[n-1] columns into rows
+  // padded from out_dim, and the prior and the score rows are out_dim wide
+  for (int l = 0; l < d->n_layers; l++)
+    if (d->layer_in[l] < 1 || d->layer_out[l] < 1) { set_error("jb200_dnn_create: layer %d is %d -> %d", l, d->layer_in[l], d->layer_out[l]); return JB200_ERR_ARG; }
+  if (d->in_dim != d->layer_in[0] || d->out_dim != d->layer_out[d->n_layers - 1]) {
+    set_error("jb200_dnn_create: net is %d -> %d but its layers take %d and give %d", d->in_dim, d->out_dim, d->layer_in[0], d->layer_out[d->n_layers - 1]);
+    return JB200_ERR_ARG;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (libjb200 has no CPU fallback)"); return JB200_ERR_NODEVICE; }
   if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return JB200_ERR_ARG; }
@@ -348,6 +350,9 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
     for (int i = 0; i < LOGISTIC_N; i++) { double x = (double)i / 20000.0 - 8.0; tbl[i] = (float)(1.0 / (1.0 + exp(-x))); }
     JB_CUDA(cudaMalloc(&h->d_logistic, sizeof(float) * LOGISTIC_N));
     JB_CUDA(cudaMemcpy(h->d_logistic, tbl.data(), sizeof(float) * LOGISTIC_N, cudaMemcpyHostToDevice));
+    build_addlog_table(tbl);
+    JB_CUDA(cudaMalloc(&h->d_addlog, sizeof(float) * tbl.size()));
+    JB_CUDA(cudaMemcpy(h->d_addlog, tbl.data(), sizeof(float) * tbl.size(), cudaMemcpyHostToDevice));
   }
   h->ld_logits = (d->out_dim + 3) & ~3;
   JB_CUDA(cudaFuncSetAttribute(dnn_gemm_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
@@ -404,7 +409,8 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
     JB_LAUNCH_CHECK();
     cur ^= 1;
   }
-  dnn_softmax_kernel<<<T, 256, 0, st>>>(h->d_logits, h->ld_logits, h->out_dim, h->d_prior, d_rows, row_stride);
+  dnn_softmax_kernel<<<(T + 32 * SOFTMAX_WARPS - 1) / (32 * SOFTMAX_WARPS), 32 * SOFTMAX_WARPS, 0, st>>>(h->d_logits, h->ld_logits, h->out_dim, T,
+                                                                                        h->d_prior, h->d_addlog, d_rows, row_stride);
   JB_LAUNCH_CHECK();
   return JB200_OK;
 }

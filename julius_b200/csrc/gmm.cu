@@ -54,15 +54,6 @@ __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigne
   return pack2(__fmaf_rn(lo2(a), lo2(b), lo2(c)), __fmaf_rn(hi2(a), hi2(b), hi2(c)));
 }
 
-__device__ __forceinline__ float addlog_step_exact(float y, float x, const float *__restrict__ tbl) {
-  // addlog.c:112-120
-  if (x > y) { float t = x; x = y; y = t; }
-  float tmp = __fsub_rn(x, y);
-  if ((double)tmp < JB200_LOG_ADDMIN) return y;
-  unsigned int idx = (unsigned int)__dadd_rn(__dmul_rn((double)(-tmp), 33333.3333), 0.5);
-  return __fadd_rn(y, __ldg(tbl + idx));
-}
-
 __device__ __forceinline__ float finish_exact(float lp) {
   // calc_mix.c:72-80 for a single stream with weight 1
   if (lp <= JB200_LOG_ZERO || lp == 0.0f) return JB200_LOG_ZERO;
@@ -350,15 +341,6 @@ int gmm_cd_device(const jb200_gmm *h, const int **cd_off, const int **cd_states,
   *cd_off = h->d_cd_off; *cd_states = h->d_cd_states; *method = h->iwcd_method; *nbest = h->iwcd_nbest;
   return 0;
 }
-}
-
-static void build_addlog_table(std::vector<float> &tbl) {
-  // addlog.c:39-57 -- same libm calls on the host, uploaded once
-  tbl.resize(500000);
-  for (int i = 0; i < 500000; i++) {
-    float f = -((float)15 * (float)i / (float)500000);
-    tbl[i] = (float)log(1 + exp((double)f));
-  }
 }
 
 extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, jb200_gmm **out) {

@@ -100,6 +100,30 @@ def test_product_path_fails_loudly_without_a_device():
     assert capi.lib().jb200_device_count() <= 0 or True      # the call itself must not crash
 
 
+def test_dnn_create_refuses_inconsistent_widths():
+    """jb200_dnn_create checks the net's widths before it looks for a device: an in_dim other than the first layer's
+    input, an out_dim other than the last layer's output, or a width below 1 is JB200_ERR_ARG, with or without a GPU."""
+    from util import dnn_blob
+    rng = np.random.default_rng(0)
+    w0, w1 = rng.standard_normal((8, 5)).astype(np.float32), rng.standard_normal((3, 8)).astype(np.float32)
+    good = dnn_blob([w0, w1], [np.zeros(8, np.float32), np.zeros(3, np.float32)], np.zeros(3, np.float32))
+    bad = {"in_dim": {"dnn.in_dim": 6}, "out_dim": {"dnn.out_dim": 4}, "zero_width": {"dnn.l0.out": 0, "dnn.l1.in": 0},
+           "zero_in": {"dnn.in_dim": 0, "dnn.l0.in": 0}, "zero_out": {"dnn.out_dim": 0, "dnn.l1.out": 0}}
+
+    def create(blob):
+        h = C.c_void_p()
+        rc = capi.lib().jb200_dnn_create(C.byref(desc.Descriptors(blob).dnn), 0, C.byref(h))
+        if h:
+            capi.lib().jb200_dnn_destroy(h)
+        return rc
+
+    for name, change in bad.items():
+        blob = dict(good)
+        blob.update({k: np.array([v], np.int32) for k, v in change.items()})
+        assert create(blob) == -1, name                           # JB200_ERR_ARG
+    assert create(good) in (0, -3)                               # JB200_OK, or JB200_ERR_NODEVICE without a GPU
+
+
 def test_nothing_in_the_product_imports_the_oracle():
     """oracle/ is test infrastructure: no module of julius_b200/ and none of the C/CUDA sources may reference it."""
     pkg = os.path.join(ROOT, "julius_b200")

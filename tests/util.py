@@ -68,6 +68,150 @@ def full_dnn_blob(seed=3, in_dim=528, hidden=2048, layers=7, n_out=3000):
     return b
 
 
+def dnn_blob(ws, bs, prior):
+    """A DNN blob dict (the layout of full_dnn_blob) from per-layer weights [out, in] and biases [out]."""
+    b = {"dnn.n_layers": np.array([len(ws)], np.int32), "dnn.in_dim": np.array([ws[0].shape[1]], np.int32),
+         "dnn.out_dim": np.array([ws[-1].shape[0]], np.int32), "gmm.n_states": np.array([ws[-1].shape[0]], np.int32)}
+    for i, (w, bias) in enumerate(zip(ws, bs)):
+        b[f"dnn.l{i}.in"] = np.array([w.shape[1]], np.int32)
+        b[f"dnn.l{i}.out"] = np.array([w.shape[0]], np.int32)
+        b[f"dnn.l{i}.w"] = np.ascontiguousarray(w, np.float32).ravel()
+        b[f"dnn.l{i}.b"] = np.ascontiguousarray(bias, np.float32)
+    b["dnn.state_prior"] = np.ascontiguousarray(prior, np.float32)
+    return b
+
+
+def random_prior(rng, n):
+    return np.log10(rng.dirichlet(np.full(n, 5.0))).astype(np.float32)
+
+
+# ---- designed DNNs whose output the restatement gives bit for bit (tests/test_gpu_dnn_shapes.py) -------------------
+# K2 splits every operand into bf16 hi + lo and sums hi.hi + hi.lo + lo.hi in fp32.  A value with at most 16 significant
+# bits splits exactly, and when one operand of each product is hi-only (8 bits) the dropped lo.lo term is zero.  If every
+# product and every partial sum is a multiple of one grid and stays below 2^20 grid units, each sum is exact in fp32 in
+# any order, so the logits equal the restatement's; what remains is the normaliser, which replays addlog_array.
+
+def round_sig16(a):
+    """float32 rounded to 16 significant bits (nearest, ties to even)"""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
+    u = (u + 0x7F + ((u >> 8) & 1)) & 0xFFFFFF00
+    return u.astype(np.uint32).view(np.float32)
+
+
+def softmax_designs(n, rng):
+    """Designed logit vectors of length n: flat, broad, peaked like a trained acoustic model with the peak early or late
+    in addlog_array's walk (which runs from n-1 down to 0), ties, a -1e10 entry, a 1e4 spread, clusters around the
+    LOG_ADDMIN cut.  Each value has at most 16 significant bits."""
+    def nrm(mu, s):
+        return mu + s * rng.standard_normal(n)
+
+    def put(a, idx, v):
+        a = a.copy()
+        a[idx] = v
+        return a
+
+    last = n - 1
+    two = rng.choice(n, size=min(2, n), replace=False)
+    near = -13.8155 + rng.integers(-8, 9, n) * 2.0 ** -12          # both sides of the cut, 2^-12 apart
+    cluster = np.where(rng.random(n) < 0.5, -13.7, -13.9)
+    d = {
+        "flat": np.zeros(n),
+        "n3_top15_first": put(nrm(0, 3), 0, 15.0),
+        "n3_top15_last": put(nrm(0, 3), last, 15.0),
+        "n2_top12_first": put(nrm(0, 2), 0, 12.0),
+        "top10_first_rest_n-4": put(nrm(-4, 1), 0, 10.0),
+        "top10_last_rest_n-4": put(nrm(-4, 1), last, 10.0),
+        "top0_first_rest_-13.9": put(np.full(n, -13.9), 0, 0.0),
+        "top0_last_rest_-13.9": put(np.full(n, -13.9), last, 0.0),
+        "n1": nrm(0, 1), "n3": nrm(0, 3), "n5": nrm(0, 5),
+        "two_equal_maxima": put(nrm(0, 3), two, 15.0),
+        "minus_1e10": put(nrm(0, 3), rng.integers(n), -1e10),
+        "spread_1e4": rng.uniform(-5e3, 5e3, n),
+        "clusters_-13.7_-13.9_first": put(cluster, 0, 0.0),
+        "clusters_-13.7_-13.9_last": put(cluster, last, 0.0),
+        "near_cut_first": put(near, 0, 0.0),
+        "near_cut_last": put(near, last, 0.0),
+    }
+    return {k: round_sig16(v.astype(np.float32)) for k, v in d.items()}
+
+
+def one_hot_softmax_net(n, seed):
+    """Single layer, one input per design: frame t is one-hot at t, so its logits are design t exactly (bias 0)."""
+    rng = np.random.default_rng(seed)
+    designs = softmax_designs(n, rng)
+    w = np.stack(list(designs.values()), axis=1)                  # [n, K]
+    x = np.eye(w.shape[1], dtype=np.float32)
+    return dnn_blob([w], [np.zeros(n, np.float32)], random_prior(rng, n)), x, list(designs)
+
+
+# operand patterns: (input bits, input exponent, weight bits, weight exponent); values are m * 2^-e with |m| < 2^bits
+EXACT_PATTERNS = {"hi_hi": (7, 4, 7, 6),      # both operands hi-only: hi.hi alone
+                  "lo_hi": (11, 10, 4, 2),    # inputs with lo parts: pins lo.hi
+                  "hi_lo": (4, 2, 11, 10)}    # weights with lo parts: pins hi.lo
+EXACT_LIMIT = 2 ** 20                         # grid units; fp32 has 24 bits, 4 are kept as margin
+
+
+def exact_grid_layer(rng, m_x, ax, out_dim, wb, aw, nnz=24):
+    """Weights and bias for integer inputs m_x [T, in] on the grid 2^-ax: nnz non-zero weights per output, m_w * 2^-aw
+    with 0 < |m_w| < 2^wb, bias on the product grid 2^-(ax+aw).  Returns (x, w, b); asserts the exactness bound."""
+    T, in_dim = m_x.shape
+    k = min(in_dim, nnz)
+    m_w = np.zeros((out_dim, in_dim), np.int64)
+    mag = rng.integers(1, 2 ** wb, (out_dim, k)) * rng.choice([-1, 1], (out_dim, k))
+    cols = np.argsort(rng.random((out_dim, in_dim)), axis=1)[:, :k]
+    np.put_along_axis(m_w, cols, mag, axis=1)
+    m_b = rng.integers(-2 ** 16, 2 ** 16 + 1, out_dim)
+    bound = (np.abs(m_x).astype(np.int64) @ np.abs(m_w).T).max(initial=0) + np.abs(m_b).max()
+    assert bound < EXACT_LIMIT, f"design error: sum of |x w| + |b| reaches {bound} grid units (limit {EXACT_LIMIT})"
+    x = (m_x * 2.0 ** -ax).astype(np.float32)
+    w = (m_w * 2.0 ** -aw).astype(np.float32)
+    b = (m_b * 2.0 ** -(ax + aw)).astype(np.float32)
+    assert np.array_equal(x, m_x * 2.0 ** -ax) and np.array_equal(w, m_w * 2.0 ** -aw)
+    return x, w, b
+
+
+def exact_grid_net(in_dim, out_dim, T, pattern, seed):
+    """A single-layer exact-grid net and inputs (see EXACT_PATTERNS) -> (blob, x)."""
+    rng = np.random.default_rng(seed)
+    xb, ax, wb, aw = EXACT_PATTERNS[pattern]
+    m_x = rng.integers(-(2 ** xb - 1), 2 ** xb, (T, in_dim))
+    x, w, b = exact_grid_layer(rng, m_x, ax, out_dim, wb, aw)
+    return dnn_blob([w], [b], random_prior(rng, out_dim)), x
+
+
+def addlog_table_np():
+    """addlog.c:39-57 in numpy"""
+    f = -(np.float32(15) * np.arange(500000, dtype=np.float32) / np.float32(500000))
+    return np.log(1 + np.exp(f.astype(np.float64))).astype(np.float32)
+
+
+def addlog_array_np(a, tbl):
+    """addlog_array (addlog.c:102-123) on every row of a [T, N] float32, in float32 with the same double promotions"""
+    a = np.asarray(a, np.float32)
+    y = np.full(a.shape[0], -1000000.0, np.float32)
+    for n in range(a.shape[1] - 1, -1, -1):
+        x = a[:, n]
+        hi, lo = np.maximum(x, y), np.minimum(x, y)
+        tmp = lo - hi
+        keep = tmp.astype(np.float64) >= -13.815510558
+        idx = np.where(keep, (-tmp).astype(np.float64) * 33333.3333 + 0.5, 0).astype(np.uint32)
+        y = np.where(keep, hi + tbl[idx], hi)
+    return y
+
+
+def single_layer_scores_np(blob, x, tbl):
+    """Exact float64 logits of a single-layer net (asserted representable in float32), then addlog_array and the prior
+    line of calc_dnn.c:862-865 in numpy"""
+    n, k = int(blob["dnn.out_dim"][0]), int(blob["dnn.in_dim"][0])
+    w = blob["dnn.l0.w"].reshape(n, k).astype(np.float64)
+    logits = x.astype(np.float64) @ w.T + blob["dnn.l0.b"].astype(np.float64)
+    l32 = logits.astype(np.float32)
+    assert np.array_equal(l32.astype(np.float64), logits), "design error: the logits are not exact in float32"
+    lp = addlog_array_np(l32, tbl)
+    out = 0.434294482 * (l32 - lp[:, None]).astype(np.float64) - blob["dnn.state_prior"].astype(np.float64)
+    return out.astype(np.float32)
+
+
 # A golden model is stored whole (model.jb2m), or, where that file would exceed 1 MB, as model_delta.npz: the entries that
 # differ from the model of the golden case meta["base"] (all of them when there is no base), compressed; meta["drop"] lists
 # the base's entries the model does not have.
