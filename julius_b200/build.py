@@ -23,7 +23,7 @@ def up_to_date() -> bool:
     if not os.path.exists(LIB):
         return False
     t = os.path.getmtime(LIB)
-    deps = sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + glob.glob(os.path.join(HERE, "csrc", "*.inc")) + glob.glob(os.path.join(ROOT, "include", "*.h"))
+    deps = sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + glob.glob(os.path.join(ROOT, "include", "*.h"))
     return all(os.path.getmtime(d) <= t for d in deps)
 
 

@@ -3,9 +3,9 @@
 // Stands in for libjulius/src/beam.c get_back_trellis_init/_proceed/_end + finalize_1st_pass
 // (:1825, :2663, :3052, :3133), outprob_style (outprob_style.c:354-494), the factoring look-ups
 // (factoring_sub.c:942-1143, ngram_access.c:249-305) and the word-trellis store/sort
-// (backtrellis.c:190-267,438-478), stock "fast" switches: N-gram LMs on normal trees (beam_kernel, body in
-// beam_frames.inc) and multipath trees (beam_kernel_mp); DFA grammars on the category tree (beam_kernel_grammar = the
-// same body with the three grammar-mode differences compiled in).
+// (backtrellis.c:190-267,438-478), stock "fast" switches: N-gram LMs on normal trees (beam_kernel<false, .>) and
+// multipath trees (beam_kernel_mp); DFA grammars on the category tree (beam_kernel<true, .> = the same body with the
+// three grammar-mode differences compiled in).
 //
 // Why this is not a transliteration.  The reference walks the survivors of frame t-1 one by one
 // and lets each arc "propagate" into a per-node slot; ties are won by whoever arrived first, new
@@ -82,7 +82,7 @@ struct SlotView {
 static constexpr int CHUNK_FIRST = 1, CHUNK_FINAL = 2, CHUNK_SKIP = 4;   // SKIP: nothing to do for this utterance in this launch
 struct ChunkDesc { int t0, t1, flags, row_base; };   // score row of frame t: rows + (row_base + t) * row_stride
 struct UttState {
-  int ns, natoms, tnum_prev, slots_clean, overflow, stopped, cur, n_left;
+  int ns, natoms, tnum_prev, slots_clean, overflow, stopped, cur;   // cur: the multipath kernel's current token list
   float thr; int t_done;
   // best partial sentence at the last frame done (bt_current_max, beam.c:876-921): filled when BeamParams.interim is set
   int interim_frame, interim_nwords; float interim_score; int pad_;
@@ -119,7 +119,6 @@ struct BeamParams {
   long long *prof;            // [n_utts][8] cycle counters per phase, or NULL
   unsigned *bitmask; int *wordpre;   // per-utterance arrival-order bitmask [maxbits/32] and its word prefix counts
   unsigned long long *misspec_counter;        // beam-cut counters, see jb200_decoder_create
-  int check_heap;                              // JB200_CHECK_HEAP=1: check every cut against the plain sequential replay
   unsigned long long *lmc; int lmc_bits;      // memo of max_successor_prob, 2^lmc_bits entries (0 = off)
   int maxt, maxc, maxw, maxbits;
   // token sets too large for shared memory (wide beams on large trees): the heap-select array lives in global memory
@@ -843,25 +842,30 @@ __device__ int heap_select_closed(unsigned long long *heap, const int n, const i
 }
 
 
+// trace_backptr (beam.c:253-301): the word ids of the atoms from `a` back to the sentence start, in sentence order, into
+// w[0..MAX_WORDS); returns their count.  One thread.
+__device__ int trace_backptr(const jb200_atom *atoms, int a, int *w) {
+  int n = 0;
+  w[n++] = atoms[a].wid;
+  while (atoms[a].begintime > 0) {
+    a = atoms[a].last;
+    if (a < 0 || n >= MAX_WORDS) break;
+    w[n++] = atoms[a].wid;
+  }
+  for (int i = 0; i < n / 2; i++) { const int x = w[i]; w[i] = w[n - 1 - i]; w[n - 1 - i] = x; }
+  return n;
+}
+
 // bt_current_max (beam.c:876-921): the best trellis word among those stored in the frame just done (raw atoms lo..hi-1,
 // end time frame-1), the most recently stored one on a tie (the reference walks its list newest first and keeps the
-// first maximum), traced back to the sentence start (trace_backptr, beam.c:253-301).  One thread.
+// first maximum), traced back to the sentence start.  One thread.
 __device__ void interim_best(const BeamParams &p, const int u, const jb200_atom *araw, const int lo, const int hi, const int frame) {
   UttState *st = p.state + u;
   int best = -1; float mx = JB200_LOG_ZERO;
   for (int a = hi - 1; a >= lo; a--) if (mx < araw[a].backscore) { mx = araw[a].backscore; best = a; }
   st->interim_frame = frame - 1;
   if (best < 0) { st->interim_nwords = 0; st->interim_score = JB200_LOG_ZERO; return; }
-  int *w = p.interim_words + (size_t)u * MAX_WORDS;
-  int n = 0, a = best;
-  w[n++] = araw[a].wid;
-  while (araw[a].begintime > 0) {
-    a = araw[a].last;
-    if (a < 0 || n >= MAX_WORDS) break;
-    w[n++] = araw[a].wid;
-  }
-  for (int i = 0; i < n / 2; i++) { const int x = w[i]; w[i] = w[n - 1 - i]; w[n - 1 - i] = x; }
-  st->interim_nwords = n; st->interim_score = mx;
+  st->interim_nwords = trace_backptr(araw, best, p.interim_words + (size_t)u * MAX_WORDS); st->interim_score = mx;
 }
 
 // phase cycle accounting (thread 0 only; negligible cost)
@@ -941,13 +945,15 @@ __device__ __forceinline__ void beam_cut(const BeamParams &p, const CutAreas &ca
   }
 }
 
-// finalize_1st_pass (bt_relocate_rw + bt_sort_rw, backtrellis.c:218-267,438-478) + find_1pass_result
-// (beam.c:394-424, :253-301); shared by the normal and the multipath kernel.  All threads call it.
+// finalize_1st_pass (bt_relocate_rw + bt_sort_rw, backtrellis.c:218-267,438-478) + find_1pass_result + trace_backptr; all
+// three kernels end with it.  The pass-1 result is, for an N-gram (beam.c:394-424), the </s> atom of the latest end frame
+// that holds one; for a grammar (beam.c:435-458), the best atom of the latest end frame that holds any, whatever its word.
+// All threads call it.
+template <bool GRAMMAR>
 __device__ __forceinline__ void finalize_utt(const BeamParams &p, const int u, const int tid, const int T, jb200_atom *araw, int *newidx,
                                              const int *group0, jb200_utt_result *res, int *words,
                                              int &s_natoms, int &s_overflow, int &s_found, long long &s_outbase,
                                              long long *s_prof, long long &s_tprev) {
-  // ================= finalize_1st_pass: bt_relocate_rw + bt_sort_rw (backtrellis.c:218-267,438-478) ====
   // group g = atoms with end frame g (raw atoms are grouped by creation frame already);
   // inside a group order by word id (unique per group in this build: one token per node).
   const int natoms = s_natoms;
@@ -974,8 +980,8 @@ __device__ __forceinline__ void finalize_utt(const BeamParams &p, const int u, c
     jb200_atom me = araw[a];
     me.last = (me.last < 0) ? -1 : newidx[me.last];
     p.atoms_out[ob + newidx[a]] = me;
-    // find_1pass_result (beam.c:394-424): the latest end frame holding a </s> atom
-    if (me.wid == p.tail_silwid && me.backscore > JB200_LOG_ZERO) atomicMax(&s_found, me.endtime);
+    // the result's end frame
+    if ((GRAMMAR || me.wid == p.tail_silwid) && me.backscore > JB200_LOG_ZERO) atomicMax(&s_found, me.endtime);
   }
   __threadfence_block();
   __syncthreads();
@@ -985,26 +991,23 @@ __device__ __forceinline__ void finalize_utt(const BeamParams &p, const int u, c
     const int last_time = s_found;
     if (kept == 0 || last_time < 0) status = -1;
     else {
-      // the unique </s> atom of group last_time
+      const jb200_atom *const atoms = p.atoms_out + ob;
       const int lo = group0[last_time], hi = group0[last_time + 1];
       int best = -1;
-      for (int b = lo; b < hi; b++) {
-        const jb200_atom x = p.atoms_out[ob + b];
-        if (x.wid == p.tail_silwid && x.backscore > JB200_LOG_ZERO) { best = b; break; }
+      if constexpr (GRAMMAR) {
+        float maxscore = JB200_LOG_ZERO;
+        for (int b = lo; b < hi; b++) {                    // rw[last_time][] order = word id order; strict '<' keeps the first maximum
+          const jb200_atom x = atoms[b];
+          if (maxscore < x.backscore) { maxscore = x.backscore; best = b; }
+        }
+      } else {
+        for (int b = lo; b < hi; b++) {                    // the group's only </s> atom
+          const jb200_atom x = atoms[b];
+          if (x.wid == p.tail_silwid && x.backscore > JB200_LOG_ZERO) { best = b; break; }
+        }
       }
       if (best < 0) status = -1;
-      else {
-        // trace_backptr (beam.c:253-301)
-        int tmp[MAX_WORDS]; int n = 0; int a = best;
-        tmp[n++] = p.atoms_out[ob + a].wid;
-        while (p.atoms_out[ob + a].begintime > 0) {
-          a = p.atoms_out[ob + a].last;
-          if (a < 0 || n >= MAX_WORDS) break;
-          tmp[n++] = p.atoms_out[ob + a].wid;
-        }
-        for (int i = 0; i < n; i++) words[i] = tmp[n - i - 1];
-        nw = n; score = p.atoms_out[ob + best].backscore;
-      }
+      else { nw = trace_backptr(atoms, best, words); score = atoms[best].backscore; }
     }
     jb200_utt_result r;
     r.status = status; r.n_frames = T; r.n_atoms = kept; r.n_words = nw; r.score = score;
@@ -1015,92 +1018,536 @@ __device__ __forceinline__ void finalize_utt(const BeamParams &p, const int u, c
   }
 }
 
-// The same for grammar (DFA) mode: the pass-1 result is the best atom of the last frame that holds any
-// (find_1pass_result, beam.c:435-458), whatever its word.
-__device__ __forceinline__ void finalize_utt_grammar(const BeamParams &p, const int u, const int tid, const int T, jb200_atom *araw, int *newidx,
-                                             const int *group0, jb200_utt_result *res, int *words,
-                                             int &s_natoms, int &s_overflow, int &s_found, long long &s_outbase,
-                                             long long *s_prof, long long &s_tprev) {
-  // ================= finalize_1st_pass: bt_relocate_rw + bt_sort_rw (backtrellis.c:218-267,438-478) ====
-  // group g = atoms with end frame g (raw atoms are grouped by creation frame already);
-  // inside a group order by word id (unique per group in this build: one token per node).
-  const int natoms = s_natoms;
-  for (int a = tid; a < natoms; a += BEAM_THREADS) {
-    const jb200_atom me = araw[a];
-    const int lo = group0[me.endtime], hi = group0[me.endtime + 1];
-    int rank = 0;
-    for (int b = lo; b < hi; b++) rank += (araw[b].wid < me.wid) ? 1 : 0;
-    newidx[a] = lo + rank;
-  }
-  if (tid == 0) {
-    if (p.atoms_in_place) s_outbase = p.atom_off[u];        // streams: each utterance keeps its own output region
-    else {
-      unsigned long long base = atomicAdd(p.atom_counter, (unsigned long long)natoms);
-      if ((long long)(base + natoms) > p.atoms_out_cap) { s_overflow = 1; s_outbase = -1; }
-      else s_outbase = (long long)base;
-    }
-  }
-  __syncthreads();
-  const long long ob = s_outbase;
-  const bool can_write = (ob >= 0);
-  const int kept = can_write ? natoms : 0;
-  for (int a = tid; a < kept; a += BEAM_THREADS) {
-    jb200_atom me = araw[a];
-    me.last = (me.last < 0) ? -1 : newidx[me.last];
-    p.atoms_out[ob + newidx[a]] = me;
-    // find_1pass_result (beam.c:394-424): the latest end frame holding a </s> atom
-    if (me.backscore > JB200_LOG_ZERO) atomicMax(&s_found, me.endtime);
-  }
-  __threadfence_block();
-  __syncthreads();
+// ---- what the normal-tree and the multipath kernel share ------------------------------------------------------------
+// Utterance u's part of the per-utterance work areas.  The isolated-root table is sized with the host's stride
+// max(n_iso, n_isoarc, 1) (n_isoarc = 0 on normal trees).
+struct UttAreas {
+  Tok *tok0; int *ord0; SlotView slots; Cand *cand; CandB *candb; IsoCand *iso; WEnd *wend;
+  Tok *surv;                            // normal trees: the survivors of the previous frame, in visiting order
+  unsigned *bits; int *wpre;
+  jb200_atom *araw; int *newidx; int atom_cap;
+  int *group0;                          // [T+1]: first raw atom of end-frame group g
+  int *counts; jb200_utt_result *res; int *words;
+};
+__device__ __forceinline__ UttAreas utt_areas(const BeamParams &p, const int u) {
+  const int f_begin = p.frame_off[u];   // only addresses the work areas: a launch covers the frames its ChunkDesc names
+  const long long a0 = p.atom_off[u];
+  UttAreas a;
+  a.tok0 = p.tok + (size_t)u * 2 * p.maxt;
+  a.ord0 = p.order + (size_t)u * 2 * p.maxt;
+  a.slots = SlotView{p.slots + (size_t)u * p.n_nodes};
+  a.cand = p.cand + (size_t)u * p.maxc;
+  a.candb = p.candb + (size_t)u * p.maxc;
+  a.surv = p.surv + (size_t)u * (p.beam + 2);
+  a.iso = p.iso + (size_t)u * max(max(p.n_iso, p.n_isoarc), 1);
+  a.wend = p.wend + (size_t)u * p.maxw;
+  a.bits = p.bitmask + (size_t)u * (p.maxbits >> 5);
+  a.wpre = p.wordpre + (size_t)u * (p.maxbits >> 5);
+  a.atom_cap = (int)(p.atom_off[u + 1] - a0);
+  a.araw = p.atoms_raw + a0;
+  a.newidx = p.newidx + a0;
+  a.group0 = p.group0 + (size_t)f_begin + u;
+  a.counts = p.counts + (size_t)f_begin * 2;
+  a.res = p.results + u;
+  a.words = p.words + (size_t)u * MAX_WORDS;
+  return a;
+}
 
-  if (tid == 0) {
-    int status = 0, nw = 0; float score = 0.0f;
-    const int last_time = s_found;
-    if (kept == 0 || last_time < 0) status = -1;
-    else {
-      // the unique </s> atom of group last_time
-      const int lo = group0[last_time], hi = group0[last_time + 1];
-      int best = -1; float maxscore = JB200_LOG_ZERO;
-      for (int b = lo; b < hi; b++) {                      // rw[last_time][] order = word id order; strict '<' keeps the first maximum
-        const jb200_atom x = p.atoms_out[ob + b];
-        if (maxscore < x.backscore) { maxscore = x.backscore; best = b; }
-      }
-      if (best < 0) status = -1;
-      else {
-        // trace_backptr (beam.c:253-301)
-        int tmp[MAX_WORDS]; int n = 0; int a = best;
-        tmp[n++] = p.atoms_out[ob + a].wid;
-        while (p.atoms_out[ob + a].begintime > 0) {
-          a = p.atoms_out[ob + a].last;
-          if (a < 0 || n >= MAX_WORDS) break;
-          tmp[n++] = p.atoms_out[ob + a].wid;
-        }
-        for (int i = 0; i < n; i++) words[i] = tmp[n - i - 1];
-        nw = n; score = p.atoms_out[ob + best].backscore;
-      }
+// tid 0: the scalars a kernel keeps in shared memory, fresh at the utterance's first chunk, else as the last launch parked them
+__device__ __forceinline__ void resume_scalars(const bool first, const UttState *ust, int &natoms, int &overflow, float &thr, int &ns,
+                                               long long *prof) {
+  if (first) { natoms = 0; overflow = 0; thr = JB200_LOG_ZERO; ns = 0; for (int k = 0; k < 8; k++) prof[k] = 0; }
+  else { natoms = ust->natoms; overflow = ust->overflow; thr = ust->thr; ns = ust->ns; for (int k = 0; k < 8; k++) prof[k] = ust->prof[k]; }
+}
+
+// tid 0, at the end of a chunk that is not the utterance's last: park those scalars (everything else already lives in the
+// utterance's global work area) and, when asked, the best partial sentence.  The word ends of frame T-1 were stored in
+// frame T-1 (multipath: in half B of frame T-1), with end time T-2.
+__device__ __forceinline__ void park_scalars(const BeamParams &p, const int u, const UttAreas &ua, const int T, const int natoms,
+                                             const int overflow, const float thr, const int ns, const int cur, const int tnum_prev,
+                                             const int stopped, const bool slots_clean, long long *prof, const long long tprev) {
+  UttState *const ust = p.state + u;
+  ust->natoms = natoms; ust->overflow = overflow; ust->thr = thr; ust->ns = ns; ust->cur = cur;
+  ust->tnum_prev = tnum_prev; ust->stopped = stopped; ust->slots_clean = slots_clean ? 1 : 0;
+  ust->t_done = T;
+  long long _n = clock64(); prof[7] += _n - tprev;
+  for (int k = 0; k < 8; k++) ust->prof[k] = prof[k];
+  if (p.interim) interim_best(p, u, ua.araw, (T >= 2 && stopped < 0) ? ua.group0[T - 2] : natoms, natoms, T - 1);
+}
+
+// save_trellis (beam.c:2209): the trellis word of word-end token tk, ending at frame endtime
+__device__ __forceinline__ jb200_atom trellis_atom(const Tok &tk, const int wid, const int endtime, const jb200_atom *araw) {
+  jb200_atom a;
+  a.wid = wid; a.backscore = tk.score;
+  a.begintime = (tk.tre < 0 ? -1 : araw[tk.tre].endtime) + 1;
+  a.endtime = endtime; a.last = tk.tre; a.lscore = tk.lscore;
+  return a;
+}
+
+// Word-internal candidate k of token tk on node nr (beam_intra_word_core, beam.c:2004-2177): k = 0 the self-loop if there
+// is one, then the arc to nr.next if there is one, then the explicit arcs.  Entering another node that carries a 1-gram
+// factoring id replaces the token's LM term by the node's.  out = the destination node's output.  beam_kernel_mp keeps
+// its own copy of this arc (phase A2), which reads scid alone: keep the two in step.
+struct IntraArc { int next; float score, lscore; int out; };
+__device__ __forceinline__ IntraArc intra_arc(const BeamParams &p, const Tok &tk, const NodeRec &nr, const int k) {
+  int next; float pa;
+  const int has_self = (nr.self_a != JB200_LOG_ZERO), has_next = (nr.next_a != JB200_LOG_ZERO);
+  if (has_self && k == 0) { next = tk.node; pa = nr.self_a; }
+  else if (has_next && k == has_self) { next = nr.next; pa = nr.next_a; }
+  else { const int a = k - has_self - has_next; next = __ldg(p.arc_to + nr.arc_off + a); pa = __ldg(p.arc_a + nr.arc_off + a); }
+  float tmpsum = tk.score + pa;
+  float lsc = JB200_LOG_ZERO;
+  int out_next = nr.out;
+  if (next != tk.node) {
+    const int2 so = __ldg(reinterpret_cast<const int2 *>(&p.nodes[next].scid));
+    const int scid = so.x;
+    out_next = so.y;
+    if (scid != 0) {
+      lsc = max_successor_prob(p, tk.cword, scid) * p.lm_weight + p.lm_penalty;
+      tmpsum -= tk.lscore;
+      tmpsum += lsc;
     }
-    jb200_utt_result r;
-    r.status = status; r.n_frames = T; r.n_atoms = kept; r.n_words = nw; r.score = score;
-    r.atom_offset = ob; r.word_offset = u * MAX_WORDS; r.overflow = s_overflow;
-    *res = r;
-    PROF_MARK(7);
-    if (p.prof) for (int k = 0; k < 8; k++) p.prof[(size_t)u * 8 + k] = s_prof[k];
   }
+  if (lsc == JB200_LOG_ZERO) lsc = tk.lscore;
+  return IntraArc{next, tmpsum, lsc, out_next};
+}
+
+// creation order (create_token numbering, beam.c:1147-1162): wpre[w] = the creators marked in bits[0..w); returns their
+// total.  All threads call it; no barrier after the last wpre write (none at all when nwords == 0).
+__device__ __forceinline__ int rank_creators(const unsigned *bits, int *wpre, const int nwords, int *s_warp) {
+  int carry = 0;
+  for (int w0 = 0; w0 < nwords; w0 += BEAM_THREADS) {
+    const int w = w0 + (int)threadIdx.x;
+    const int cnt = (w < nwords) ? __popc(__ldcg(bits + w)) : 0;
+    int tot;
+    const int ex = block_excl_scan(cnt, s_warp, &tot);
+    if (w < nwords) wpre[w] = carry + ex;
+    carry += tot;
+  }
+  return carry;
+}
+
+// tid 0, end of frame t: its created and surviving token counts, and the next frame's score envelope (the best score
+// created in the frame less prune_width; LOG_ZERO when off or when nothing was created)
+__device__ __forceinline__ void end_frame(const BeamParams &p, int *counts, const int t, const int ncre, const int ns_new,
+                                          const unsigned pmaxkey, int &ns, float &thr) {
+  counts[2 * t] = ncre; counts[2 * t + 1] = ns_new;
+  ns = ns_new;
+  if (p.prune_width >= 0.0f && pmaxkey != 0u) {
+    const unsigned b = (pmaxkey & 0x80000000u) ? (pmaxkey & 0x7fffffffu) : ~pmaxkey;
+    thr = __uint_as_float(b) - p.prune_width;
+  } else thr = JB200_LOG_ZERO;
+}
+
+// Self-check of a heap select (JB200_CHECK_HEAP, compiled into the CHECK instantiations of the kernels only): the plain
+// sequential select (heap_build + heap_extract_seq) of the select's input chk[1..n], compared with what the kernel made --
+// the whole arrangement heap[1..n] (multipath select #1: select #2 starts from it), or, with heap == nullptr, the survivors
+// in visiting order ordn[0..need) (the normal kernels' cut, multipath select #2).  Overflow code 4 on a difference.  With
+// tok != nullptr the input is first rebuilt from the tokens in creation order (chk may then be the cut's own heap array,
+// dead after the cut).  With overflow == nullptr it only copies heap[1..n] to chk (the input of multipath select #2, which
+// the cut destroys).  All threads call it.
+__device__ __noinline__ void check_select(unsigned long long *chk, const int n, const int need, const Tok *tok,
+                                          const unsigned long long *heap, const int *ordn, int *overflow) {
+  if (!overflow) {
+    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) chk[h] = heap[h];
+    __syncthreads();
+    return;
+  }
+  const bool upward = (need < n - need);
+  __syncthreads();
+  if (tok) for (int r = threadIdx.x; r < n; r += BEAM_THREADS) chk[r + 1] = ((unsigned long long)(unsigned)r << 32) | __float_as_uint(tok[r].score);
+  __syncthreads();
+  if (upward) { heap_build<true>(chk, n); heap_extract_seq<true>(chk, n, need); }
+  else { heap_build<false>(chk, n); heap_extract_seq<false>(chk, n, n - need); }
+  bool bad = false;
+  if (heap) {
+    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) bad |= (chk[h] != heap[h]);
+  } else {
+    const int start = upward ? n - need : 0;
+    for (int k = threadIdx.x; k < need; k += BEAM_THREADS) bad |= (ordn[k] != (int)(chk[start + k + 1] >> 32));
+  }
+  if (bad) *overflow = 4;
+  __syncthreads();
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------
 static constexpr int BEAM_MINBLOCKS = 4;
-#define BEAM_KERNEL_NAME beam_kernel
-#define BEAM_GRAMMAR 0
-#include "beam_frames.inc"
-#undef BEAM_KERNEL_NAME
-#undef BEAM_GRAMMAR
-#define BEAM_KERNEL_NAME beam_kernel_grammar
-#define BEAM_GRAMMAR 1
-#include "beam_frames.inc"
-#undef BEAM_KERNEL_NAME
-#undef BEAM_GRAMMAR
+// The normal-tree kernel, for an N-gram (1-gram factoring, bigram rows) or, GRAMMAR, a DFA grammar on the category tree.
+// The grammar differs in three places: the frame-0 tokens, the inter-word LM term and the pass-1 result (finalize_utt).
+// CHECK: the JB200_CHECK_HEAP build (the self-check stays out of the shipped kernels' register budget).
+template <bool GRAMMAR, bool CHECK>
+__global__ void __launch_bounds__(BEAM_THREADS, BEAM_MINBLOCKS)
+beam_kernel(const BeamParams p) {
+  const int u = blockIdx.x;
+  const int tid = threadIdx.x;
+  // this launch covers frames [ck.t0, ck.t1) of the utterance (ChunkDesc)
+  const ChunkDesc ck = p.chunk[u];
+  if (ck.flags & CHUNK_SKIP) return;
+  const bool ck_first = (ck.flags & CHUNK_FIRST) != 0, ck_final = (ck.flags & CHUNK_FINAL) != 0;
+  const UttState *const ust = p.state + u;
+  const int T = ck.t1;                               // frames so far; the utterance's length when ck_final
+  const int MAXT = p.maxt, MAXC = p.maxc, MAXW = p.maxw;
+
+  const CutAreas ca = cut_areas(p);
+  unsigned long long *const heap = ca.heap;
+  int *const offs = ca.offs;                          // [beam+2] candidate payload offsets per survivor
+  int *const poff = offs + (p.beam + 2);              // [beam+2] arrival-order bit positions per survivor
+  __shared__ int s_warp[NWARP + 1];
+  __shared__ int s_E, s_natoms, s_ns, s_overflow, s_found;
+  __shared__ unsigned s_pmaxkey;
+  __shared__ unsigned long long s_webest;
+  __shared__ float s_thr;
+  __shared__ long long s_outbase;
+  __shared__ long long s_prof[8], s_tprev;
+
+  const UttAreas ua = utt_areas(p, u);
+
+  if (tid == 0) {
+    s_found = -1; s_tprev = clock64();
+    resume_scalars(ck_first, ust, s_natoms, s_overflow, s_thr, s_ns, s_prof);
+  }
+  __syncthreads();
+
+  if constexpr (GRAMMAR) {
+  // ================= frame 0: init_nodescore, grammar branch (beam.c:1669-1760): one token per sentence-initial
+  // word (duplicates of a shared first node were dropped when the list was made); n_init <= beam, so the first
+  // sort_token_no_order (:1883) leaves them in creation order
+  if (T > 0 && ck_first) {
+    const float *row0 = p.rows + (size_t)ck.row_base * p.row_stride;
+    for (int i = tid; i < p.n_init; i += BEAM_THREADS) {
+      const int node = __ldg(p.init_node + i);
+      Tok tk;
+      tk.lscore = __ldg(p.init_lscore + i); tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = node;
+      tk.score = outprob_style(p, row0, p.nodes[node].out, -1) + tk.lscore;
+      ua.tok0[i] = tk;
+      ua.surv[i] = tk;
+      ua.ord0[i] = i;
+    }
+    if (tid == 0) { s_ns = p.n_init; ua.counts[0] = p.n_init; ua.counts[1] = p.n_init; }
+  }
+  } else {
+  // ================= frame 0: init_nodescore (beam.c:1631-1665) + first sort (:1883) =================
+  if (T > 0 && ck_first && tid == 0) {
+    const int node = p.head_node;
+    const NodeRec nr = p.nodes[node];
+    Tok tk;
+    float ll = (nr.scid != 0) ? max_successor_prob(p, -1, nr.scid) : 0.0f;
+    ll = ll * p.lm_weight + p.lm_penalty;
+    tk.lscore = ll; tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = node;
+    tk.score = outprob_style(p, p.rows + (size_t)ck.row_base * p.row_stride, nr.out, -1) + ll;
+    ua.tok0[0] = tk;
+    ua.surv[0] = tk;
+    ua.ord0[0] = 0;
+    s_ns = 1;
+    ua.counts[0] = 1; ua.counts[1] = 1;
+  }
+  }
+  __syncthreads();
+
+  int tnum_prev = ck_first ? ((T > 0) ? (GRAMMAR ? p.n_init : 1) : 0) : ust->tnum_prev;      // tokens created in the previous frame (clear phase)
+  int stopped = ck_first ? -1 : ust->stopped;       // frame at which the beam ran empty (beam.c:3012-3015), -1 = alive
+  bool slots_clean = ck_first ? false : (ust->slots_clean != 0);   // the previous frame's node slots were already reset under its beam cut
+
+  // ================= frames 1..T-1: get_back_trellis_proceed (beam.c:2663-3019) =================
+  for (int t = max(ck.t0, 1); t < T && stopped < 0; t++) {
+    // one token list is enough here: the survivors of t-1 live on in `ua.surv` (compact, in visiting order), so frame t's
+    // tokens may overwrite frame t-1's -- half the per-utterance token footprint in L2 (the multipath kernel still
+    // reads the old list through its order array and keeps two)
+    Tok *const tn = ua.tok0;
+    int *const ordn = ua.ord0;
+    const int ns = s_ns;
+    const float thr = s_thr;
+    const float *row = p.rows + (size_t)((long long)ck.row_base + t) * p.row_stride;
+
+    // ---- P0: clear_tokens (beam.c:1122): reset the node slots used by frame t-1 (normally done already
+    //          under that frame's beam cut, see beam_cut)
+    if (!slots_clean) SlotClear{ua.tok0, tnum_prev, ua.slots}.run(tid, BEAM_THREADS);
+    slots_clean = false;
+    if (tid == 0) { s_webest = 0ull; s_pmaxkey = 0u; ua.group0[t - 1] = s_natoms; }
+    __syncthreads();
+    PROF_MARK(0);
+
+    // ---- P1: per survivor: candidate counts, word ends, trellis atoms (save_trellis, beam.c:2209)
+    int cand_total, nbits;
+    {
+      int carry_c = 0, carry_a = s_natoms, carry_w = 0;
+      for (int j0 = 0; j0 < ns; j0 += BEAM_THREADS) {
+        const int j = j0 + tid;
+        int nin = 0, is_we = 0, is_tr = 0;
+        Tok tk; NodeRec nr;
+        if (j < ns) {
+          tk = ua.surv[j];
+          nr = p.nodes[tk.node];
+          const bool valid = (tk.score > JB200_LOG_ZERO) && !(tk.score < thr);
+          if (valid) {
+            nin = (nr.self_a != JB200_LOG_ZERO) + (nr.next_a != JB200_LOG_ZERO) + nr.arc_n;
+            if (nr.stend >= 0) { is_we = 1; is_tr = (nr.stend != p.tail_silwid); }
+          }
+        }
+        int tot_c, tot_a, tot_w;
+        const int oc = block_excl_scan(nin, s_warp, &tot_c);
+        const int oa = block_excl_scan(is_we, s_warp, &tot_a);
+        const int ow = block_excl_scan(is_tr, s_warp, &tot_w);
+        if (j < ns) {
+          offs[j] = carry_c + oc;
+          // arrival-order position of this survivor's first candidate: its word-internal arcs,
+          // then (for a word end that may continue) one slot per isolated root
+          poff[j] = carry_c + oc + (carry_w + ow) * p.n_iso;
+          if (is_we) {
+            const int ai = carry_a + oa;
+            if (ai < ua.atom_cap) ua.araw[ai] = trellis_atom(tk, nr.stend, t - 1, ua.araw);
+            else s_overflow = 1;
+            if (is_tr) {
+              const int wi = carry_w + ow;
+              if (wi < MAXW && ai < ua.atom_cap) {
+                WEnd w;
+                const int sword = nr.stend;
+                const int transp = p.is_transp[sword];
+                w.j = j; w.atom = ai; w.last_word = transp ? tk.cword : sword;
+                w.base = tk.score + __ldg(p.wordend_a + sword);
+                w.transp2 = (transp && tk.cword >= 0 && p.is_transp[tk.cword]) ? 1 : 0;
+                w.nintra = nin;
+                ua.wend[wi] = w;
+                if (w.base > JB200_LOG_ZERO)   // beam.c:2308 keeps the FIRST maximum
+                  atomicMax(&s_webest, ((unsigned long long)fkey(w.base) << 32) | (unsigned)(~(unsigned)wi));
+              } else s_overflow = 1;
+            }
+          }
+        }
+        carry_c += tot_c; carry_a += tot_a; carry_w += tot_w;
+      }
+      cand_total = carry_c;
+      nbits = carry_c + carry_w * p.n_iso + p.n_shared;
+      if (tid == 0) { offs[ns] = carry_c; poff[ns] = carry_c + carry_w * p.n_iso; s_natoms = min(carry_a, ua.atom_cap); s_E = min(carry_w, MAXW); }
+      // carry_a > atom_cap: some word ends got no atom and no wend entry, and wend[0..E) would hold stale entries
+      if (cand_total > MAXC || carry_w > MAXW || nbits > p.maxbits || carry_a > ua.atom_cap) { if (tid == 0) s_overflow = 1; cand_total = 0; nbits = 0; }
+    }
+    const int nwords = (nbits + 31) >> 5;
+    for (int w = tid; w < nwords; w += BEAM_THREADS) ua.bits[w] = 0u;
+    __syncthreads();
+    PROF_MARK(1);
+    const int E = (nbits > 0) ? s_E : 0;
+
+    // ---- P2a: word-internal transitions (beam_intra_word(_core), beam.c:2004-2177), one thread per
+    //           candidate (survivors near the tree roots fan out 10-20 ways: per-survivor loops leave most
+    //           of the block idle); the owner of candidate c is found by bisection of the offsets
+    for (int c = tid; c < cand_total; c += BEAM_THREADS) {
+      int lo = 0, hi = ns;
+      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (offs[mid] <= c) lo = mid; else hi = mid; }
+      const int j = lo;
+      int k = c - offs[j];
+      const Tok tk = ua.surv[j];
+      const IntraArc ar = intra_arc(p, tk, p.nodes[tk.node], k);
+      Cand cd; cd.score = ar.score; cd.node = ar.next; cd.lscore = ar.lscore; cd.src = j;
+      ua.cand[c] = cd;
+      CandB cb; cb.tre = tk.tre; cb.cword = tk.cword; cb.tre_wid = tk.tre_wid; cb.out = ar.out;
+      ua.candb[c] = cb;
+      if (ar.score > JB200_LOG_ZERO) {
+        const unsigned seq = (unsigned)j * SEQ_LOCAL + (unsigned)k;
+        cand_atomics(ua.slots, ar.next, ar.score, seq, seq);
+      }
+    }
+    // ---- P2b: cross-word transitions into isolated roots (beam_inter_word, beam.c:2271-2517),
+    //           pre-reduced per root over this frame's word ends, visited in survivor order
+    for (int i = tid; i < p.n_iso; i += BEAM_THREADS) {
+      const int col = __ldg(p.iso_id + i);
+      float best = JB200_LOG_ZERO, bestl = 0.0f; int beste = -1, firste = -1;
+      for (int e = 0; e < E; e++) {
+        const WEnd w = ua.wend[e];
+        float lsc;
+        if constexpr (GRAMMAR) {
+        // category-pair constraint of (ending word, root's word) and the insertion penalty (beam.c:2404-2411, :2444-2450)
+        if (!__ldg(p.cp_allowed + (size_t)w.last_word * p.n_iso + col)) continue;
+        lsc = p.penalty1 + __ldg(p.cprob + w.last_word);
+        } else {
+        const float tmpprob = __ldg(p.iw + (size_t)w.last_word * p.n_iso + col);
+        lsc = tmpprob * p.lm_weight + p.lm_penalty;
+        }
+        float tmpsum = w.base;
+        tmpsum += lsc;
+        if (w.transp2) tmpsum += p.lm_penalty_trans;
+        if (tmpsum > JB200_LOG_ZERO) {
+          if (firste < 0) firste = e;
+          if (beste < 0 || best < tmpsum) { best = tmpsum; beste = e; bestl = lsc; }
+        }
+      }
+      IsoCand ic; ic.score = best; ic.e = beste; ic.lscore = bestl; ic.first_e = firste;
+      ua.iso[i] = ic;
+      if (firste >= 0) {
+        const WEnd wf = ua.wend[firste], wb = ua.wend[beste];
+        const unsigned sf = (unsigned)wf.j * SEQ_LOCAL + (unsigned)(wf.nintra + i);
+        const unsigned sw = (unsigned)wb.j * SEQ_LOCAL + (unsigned)(wb.nintra + i);
+        cand_atomics(ua.slots, __ldg(p.iso_node + i), best, sf, sw);
+      }
+    }
+    // ---- P2c: best word end -> shared (1-gram factored) roots (beam_inter_word_factoring, :2549-2616)
+    const unsigned long long webest = s_webest;
+    const bool have_we = (webest != 0ull) && (nbits > 0);
+    WEnd wbest; wbest.base = 0.0f; wbest.atom = -1; wbest.last_word = -1; wbest.transp2 = 0; wbest.j = 0; wbest.nintra = 0;
+    if (have_we) {
+      wbest = ua.wend[(unsigned)(~(unsigned)(webest & 0xffffffffu))];
+      for (int i = tid; i < p.n_shared; i += BEAM_THREADS) {
+        const float lsc = __ldg(p.shared_f + i) * p.lm_weight + p.lm_penalty;
+        float tmpsum = wbest.base;
+        tmpsum += lsc;
+        if (wbest.transp2) tmpsum += p.lm_penalty_trans;
+        if (tmpsum < thr) continue;
+        if (tmpsum > JB200_LOG_ZERO) {
+          const unsigned seq = (unsigned)ns * SEQ_LOCAL + (unsigned)i;
+          cand_atomics(ua.slots, __ldg(p.shared_node + i), tmpsum, seq, seq);
+        }
+      }
+    }
+    __syncthreads();
+    PROF_MARK(2);
+
+    // ---- P3: creators = candidates that were the first to reach their node; one bit each at the
+    //          candidate's position in sequential arrival order
+    for (int c = tid; c < cand_total; c += BEAM_THREADS) {
+      const Cand cd = ua.cand[c];
+      if (!(cd.score > JB200_LOG_ZERO)) continue;
+      const int k = c - offs[cd.src];
+      const unsigned seq = (unsigned)cd.src * SEQ_LOCAL + (unsigned)k;
+      if ((unsigned)__ldcg(ua.slots.fs(cd.node)) == seq) {
+        const int pos = poff[cd.src] + k;
+        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
+      }
+    }
+    for (int i = tid; i < p.n_iso; i += BEAM_THREADS) {
+      const IsoCand ic = ua.iso[i];
+      if (ic.first_e < 0) continue;
+      const WEnd wf = ua.wend[ic.first_e];
+      const unsigned seq = (unsigned)wf.j * SEQ_LOCAL + (unsigned)(wf.nintra + i);
+      if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.iso_node + i))) == seq) {
+        const int pos = poff[wf.j] + wf.nintra + i;
+        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
+      }
+    }
+    if (have_we) {
+      for (int i = tid; i < p.n_shared; i += BEAM_THREADS) {
+        const unsigned seq = (unsigned)ns * SEQ_LOCAL + (unsigned)i;
+        if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.shared_node + i))) == seq) {
+          const int pos = poff[ns] + i;
+          atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
+        }
+      }
+    }
+    __syncthreads();
+    PROF_MARK(3);
+
+    // ---- P4: creation order = rank of the set bits
+    int ncre = rank_creators(ua.bits, ua.wpre, nwords, s_warp);
+    if (ncre > MAXT) { if (tid == 0) s_overflow = 1; ncre = 0; }
+    __syncthreads();
+    PROF_MARK(4);
+
+    // ---- P5: materialise tokens with the winner's content, add the output probability (beam.c:2944)
+    auto materialise = [&](int pos, int node) {
+      const unsigned wbits = __ldcg(ua.bits + (pos >> 5));
+      if (!((wbits >> (pos & 31)) & 1u)) return;
+      const int r = ua.wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
+      const unsigned long long bk = __ldcg(ua.slots.bk(node));
+      const unsigned seqw = ~(unsigned)(bk & 0xffffffffu);
+      const int j = (int)(seqw >> SEQ_LOCAL_BITS), local = (int)(seqw & (SEQ_LOCAL - 1));
+      Tok nt; nt.node = node;
+      int out;
+      if (j == ns) {                                    // factoring pass
+        const float lsc = __ldg(p.shared_f + local) * p.lm_weight + p.lm_penalty;
+        float tmpsum = wbest.base; tmpsum += lsc;
+        if (wbest.transp2) tmpsum += p.lm_penalty_trans;
+        nt.score = tmpsum; nt.lscore = lsc; nt.tre = wbest.atom; nt.cword = wbest.last_word;
+        nt.tre_wid = ua.araw[wbest.atom].wid;
+        out = p.nodes[node].out;
+      } else {
+        const int c0 = offs[j], nin = offs[j + 1] - c0;
+        if (local < nin) {                              // word-internal candidate: everything travels with it
+          const Cand cd = ua.cand[c0 + local];
+          const CandB cb = ua.candb[c0 + local];
+          nt.score = cd.score; nt.lscore = cd.lscore; nt.tre = cb.tre; nt.cword = cb.cword; nt.tre_wid = cb.tre_wid;
+          out = cb.out;
+        } else {                                        // isolated-root candidate
+          const IsoCand ic = ua.iso[local - nin];
+          const WEnd w = ua.wend[ic.e];
+          nt.score = ic.score; nt.lscore = ic.lscore; nt.tre = w.atom; nt.cword = w.last_word;
+          nt.tre_wid = ua.araw[w.atom].wid;
+          out = p.nodes[node].out;
+        }
+      }
+      nt.score += outprob_style(p, row, out, nt.tre_wid);
+      tn[r] = nt;
+      heap[r + 1] = ((unsigned long long)(unsigned)r << 32) | __float_as_uint(nt.score);
+      atomicMax(&s_pmaxkey, fkey(nt.score));
+    };
+    if (ncre > 0) {
+      for (int c = tid; c < cand_total; c += BEAM_THREADS) {
+        const Cand cd = ua.cand[c];
+        if (!(cd.score > JB200_LOG_ZERO)) continue;
+        materialise(poff[cd.src] + (c - offs[cd.src]), cd.node);
+      }
+      for (int i = tid; i < p.n_iso; i += BEAM_THREADS) {
+        const IsoCand ic = ua.iso[i];
+        if (ic.first_e < 0) continue;
+        const WEnd wf = ua.wend[ic.first_e];
+        materialise(poff[wf.j] + wf.nintra + i, __ldg(p.iso_node + i));
+      }
+      if (have_we)
+        for (int i = tid; i < p.n_shared; i += BEAM_THREADS) materialise(poff[ns] + i, __ldg(p.shared_node + i));
+    }
+    __syncthreads();
+    PROF_MARK(5);
+
+    // ---- P6: beam cut = the reference's heap select (sort_token_no_order, beam.c:1492-1520)
+    const int ns_new = min(ncre, p.beam);
+    if (ncre <= p.beam) {
+      for (int k = tid; k < ns_new; k += BEAM_THREADS) ordn[k] = k;
+    } else {
+      beam_cut(p, ca, ncre, s_pmaxkey, tn, ua.slots, ordn, s_prof, s_tprev);
+      slots_clean = true;
+      // the heap array is dead after the cut: the self-check rebuilds its input there
+      if constexpr (CHECK) check_select(heap, ncre, p.beam, tn, nullptr, ordn, &s_overflow);
+    }
+    // the survivors in visiting order, compact (every thread re-reads the order entries it wrote itself)
+    for (int k = tid; k < ns_new; k += BEAM_THREADS) ua.surv[k] = tn[ordn[k]];
+    PROF_MARK(6);
+    if (tid == 0) end_frame(p, ua.counts, t, ncre, ns_new, s_pmaxkey, s_ns, s_thr);
+    tnum_prev = ncre;
+    __syncthreads();
+    if (ncre == 0) { stopped = t; break; }      // beam.c:3012-3015: no nodes left, search terminated
+  }
+
+  if (!ck_final) {
+    if (tid == 0) park_scalars(p, u, ua, T, s_natoms, s_overflow, s_thr, s_ns, 0, tnum_prev, stopped, slots_clean, s_prof, s_tprev);
+    return;
+  }
+  const int groups = (stopped >= 0) ? stopped : T;   // number of end-frame groups kept by finalize (framelen)
+
+  // ================= get_back_trellis_end (normal version, beam.c:3076-3086) =================
+  {
+    const int ns = (T > 0) ? s_ns : 0;
+    if (tid == 0 && T > 0 && groups == T) ua.group0[T - 1] = s_natoms;
+    __syncthreads();
+    int carry_a = s_natoms;
+    for (int j0 = 0; j0 < ns; j0 += BEAM_THREADS) {
+      const int j = j0 + tid;
+      int is_we = 0; Tok tk; int stend = -1;
+      if (j < ns) { tk = ua.surv[j]; stend = p.nodes[tk.node].stend; is_we = (stend >= 0); }
+      int tot;
+      const int oa = block_excl_scan(is_we, s_warp, &tot);
+      if (is_we) {
+        const int ai = carry_a + oa;
+        if (ai < ua.atom_cap) ua.araw[ai] = trellis_atom(tk, stend, T - 1, ua.araw);     // save_trellis(t = samplenum)
+        else s_overflow = 1;
+      }
+      carry_a += tot;
+    }
+    if (tid == 0) { s_natoms = min(carry_a, ua.atom_cap); ua.group0[groups] = s_natoms; }
+    // leave the node slots clean for the next utterance that uses this work area
+    if (!slots_clean) SlotClear{ua.tok0, tnum_prev, ua.slots}.run(tid, BEAM_THREADS);
+    __syncthreads();
+  }
+
+  finalize_utt<GRAMMAR>(p, u, tid, T, ua.araw, ua.newidx, ua.group0, ua.res, ua.words, s_natoms, s_overflow, s_found, s_outbase, s_prof, s_tprev);
+}
 
 // ---- the multipath kernel ----------------------------------------------------------------------------
 // get_back_trellis_proceed, MULTIPATH branch (beam.c:2752-2828, :2930-2941).  Trees of multipath models
@@ -1131,35 +1578,6 @@ __device__ __forceinline__ int select_exact(const CutAreas &ca, int n, int need,
   return start;
 }
 
-// Self-check of a multipath select (JB200_CHECK_HEAP): the plain sequential select (heap_build + heap_extract_seq) of the
-// select's input chk[1..n], compared with what the kernel made -- the whole arrangement heap[1..n] (select #1: select #2
-// starts from it), or, with heap == nullptr, the survivors in visiting order ordn[0..need) (select #2).  Overflow code 4
-// on a difference.  With tok != nullptr the input is first rebuilt from the tokens in creation order (select #1).  With
-// overflow == nullptr it only copies heap[1..n] to chk (the input of select #2, which the cut destroys).  All threads
-// call it.
-__device__ __noinline__ void check_select_mp(unsigned long long *chk, const int n, const int need, const Tok *tok,
-                                             const unsigned long long *heap, const int *ordn, int *overflow) {
-  if (!overflow) {
-    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) chk[h] = heap[h];
-    __syncthreads();
-    return;
-  }
-  const bool upward = (need < n - need);
-  if (tok) for (int r = threadIdx.x; r < n; r += BEAM_THREADS) chk[r + 1] = ((unsigned long long)(unsigned)r << 32) | __float_as_uint(tok[r].score);
-  __syncthreads();
-  if (upward) { heap_build<true>(chk, n); heap_extract_seq<true>(chk, n, need); }
-  else { heap_build<false>(chk, n); heap_extract_seq<false>(chk, n, n - need); }
-  bool bad = false;
-  if (heap) {
-    for (int h = 1 + (int)threadIdx.x; h <= n; h += BEAM_THREADS) bad |= (chk[h] != heap[h]);
-  } else {
-    const int start = upward ? n - need : 0;
-    for (int k = threadIdx.x; k < need; k += BEAM_THREADS) bad |= (ordn[k] != (int)(chk[start + k + 1] >> 32));
-  }
-  if (bad) *overflow = 4;
-  __syncthreads();
-}
-
 static constexpr int TOK_EXISTS = 0x40000000;
 
 // CHECK: the JB200_CHECK_HEAP build of the kernel (the self-check stays out of the shipped kernel's register budget)
@@ -1168,12 +1586,11 @@ __global__ void __launch_bounds__(BEAM_THREADS, BEAM_MINBLOCKS)
 beam_kernel_mp(const BeamParams p) {
   const int u = blockIdx.x;
   const int tid = threadIdx.x;
-  // this launch covers frames [ck.t0, ck.t1) of the utterance (ChunkDesc); f_begin only addresses its work areas
+  // this launch covers frames [ck.t0, ck.t1) of the utterance (ChunkDesc)
   const ChunkDesc ck = p.chunk[u];
   if (ck.flags & CHUNK_SKIP) return;
   const bool ck_first = (ck.flags & CHUNK_FIRST) != 0, ck_final = (ck.flags & CHUNK_FINAL) != 0;
-  UttState *const ust = p.state + u;
-  const int f_begin = p.frame_off[u];
+  const UttState *const ust = p.state + u;
   const int T = ck.t1;                               // frames so far; the utterance's length when ck_final
   const int MAXT = p.maxt, MAXC = p.maxc, MAXW = p.maxw;
 
@@ -1188,27 +1605,12 @@ beam_kernel_mp(const BeamParams p) {
   __shared__ long long s_outbase;
   __shared__ long long s_prof[8], s_tprev;
 
-  Tok *tok0 = p.tok + (size_t)u * 2 * MAXT;
-  int *ord0 = p.order + (size_t)u * 2 * MAXT;
-  const SlotView slots{p.slots + (size_t)u * p.n_nodes};
-  Cand *cand = p.cand + (size_t)u * MAXC;
-  IsoCand *iso = p.iso + (size_t)u * max(max(p.n_iso, p.n_isoarc), 1);
-  WEnd *wend = p.wend + (size_t)u * MAXW;
-  unsigned *bits = p.bitmask + (size_t)u * (p.maxbits >> 5);
-  int *wpre = p.wordpre + (size_t)u * (p.maxbits >> 5);
-  const long long a0 = p.atom_off[u];
-  const int atom_cap = (int)(p.atom_off[u + 1] - a0);
-  jb200_atom *araw = p.atoms_raw + a0;
-  int *newidx = p.newidx + a0;
-  int *group0 = p.group0 + (size_t)f_begin + u;
-  int *counts = p.counts + (size_t)f_begin * 2;
-  jb200_utt_result *res = p.results + u;
-  int *words = p.words + (size_t)u * MAX_WORDS;
+  const UttAreas ua = utt_areas(p, u);
 
   if (tid == 0) {
     s_found = -1; s_tprev = clock64();
-    if (ck_first) { s_natoms = 0; s_overflow = 0; s_thr = JB200_LOG_ZERO; s_cur = 0; s_ns = 0; for (int k = 0; k < 8; k++) s_prof[k] = 0; }
-    else { s_natoms = ust->natoms; s_overflow = ust->overflow; s_thr = ust->thr; s_cur = ust->cur; s_ns = ust->ns; for (int k = 0; k < 8; k++) s_prof[k] = ust->prof[k]; }
+    resume_scalars(ck_first, ust, s_natoms, s_overflow, s_thr, s_ns, s_prof);
+    s_cur = ck_first ? 0 : ust->cur;
   }
   __syncthreads();
 
@@ -1220,8 +1622,8 @@ beam_kernel_mp(const BeamParams p) {
     float ll = (nr.scid != 0) ? max_successor_prob(p, -1, nr.scid) : 0.0f;
     ll = ll * p.lm_weight + p.lm_penalty;
     tk.lscore = ll; tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = node; tk.score = ll;
-    tok0[0] = tk;
-    ord0[0] = 0;
+    ua.tok0[0] = tk;
+    ua.ord0[0] = 0;
     s_ns = 1;
   }
   __syncthreads();
@@ -1236,21 +1638,16 @@ beam_kernel_mp(const BeamParams p) {
   for (int t = ck.t0; t <= t_last && T > 0 && stopped < 0; t++) {
     const bool final = (t == T);
     const int cur = s_cur, nxt = cur ^ 1;
-    Tok *tl = tok0 + (size_t)cur * MAXT, *tn = tok0 + (size_t)nxt * MAXT;
-    int *ordl = ord0 + (size_t)cur * MAXT, *ordn = ord0 + (size_t)nxt * MAXT;
+    Tok *tl = ua.tok0 + (size_t)cur * MAXT, *tn = ua.tok0 + (size_t)nxt * MAXT;
+    int *ordl = ua.ord0 + (size_t)cur * MAXT, *ordn = ua.ord0 + (size_t)nxt * MAXT;
     const int ns = s_ns;
     const float thr = s_thr;
     const float *row = final ? p.rows : p.rows + (size_t)((long long)ck.row_base + t) * p.row_stride;   // the final half frame reads no scores
 
     // ---- P0: clear_tokens (normally done already under the previous frame's select #2)
-    if (!slots_clean) {
-      for (int i = tid; i < tnum_prev; i += BEAM_THREADS) {
-        const int node = tl[i].node;
-        slots.reset(node);
-      }
-    }
+    if (!slots_clean) SlotClear{tl, tnum_prev, ua.slots}.run(tid, BEAM_THREADS);
     slots_clean = false;
-    if (tid == 0) { s_webest = 0ull; s_pmaxkey = fkey(JB200_LOG_ZERO); s_hmaxkey = 0u; if (t > 0) group0[t - 1] = s_natoms; }
+    if (tid == 0) { s_webest = 0ull; s_pmaxkey = fkey(JB200_LOG_ZERO); s_hmaxkey = 0u; if (t > 0) ua.group0[t - 1] = s_natoms; }
     __syncthreads();
     PROF_MARK(0);
 
@@ -1277,7 +1674,7 @@ beam_kernel_mp(const BeamParams p) {
       if (cand_total > MAXC || cand_total > p.maxbits) { if (tid == 0) s_overflow = 1; cand_total = 0; }
     }
     int nwords = (cand_total + 31) >> 5;
-    for (int w = tid; w < nwords; w += BEAM_THREADS) bits[w] = 0u;
+    for (int w = tid; w < nwords; w += BEAM_THREADS) ua.bits[w] = 0u;
     __syncthreads();
     PROF_MARK(1);
 
@@ -1290,6 +1687,8 @@ beam_kernel_mp(const BeamParams p) {
       const int j = lo;
       int k = c - offs[j];
       const Tok tk = tl[ordl[j]];
+      // the arc of intra_arc, kept apart: that one reads (scid, out) as one 8-byte read-only load, which made this
+      // kernel 1.8 % slower on dnn60k_mp (H100 80GB HBM3, 400 W limit); here only scid is needed
       const NodeRec nr = p.nodes[tk.node];
       int next; float pa;
       const int has_self = (nr.self_a != JB200_LOG_ZERO), has_next = (nr.next_a != JB200_LOG_ZERO);
@@ -1308,10 +1707,10 @@ beam_kernel_mp(const BeamParams p) {
       }
       if (lsc == JB200_LOG_ZERO) lsc = tk.lscore;
       Cand cd; cd.score = tmpsum; cd.node = next; cd.lscore = lsc; cd.src = j;
-      cand[c] = cd;
+      ua.cand[c] = cd;
       if (tmpsum > JB200_LOG_ZERO) {
         const unsigned seq = (unsigned)j * SEQ_LOCAL + (unsigned)k;
-        cand_atomics(slots, next, tmpsum, seq, seq);
+        cand_atomics(ua.slots, next, tmpsum, seq, seq);
       }
     }
     __syncthreads();
@@ -1319,46 +1718,34 @@ beam_kernel_mp(const BeamParams p) {
 
     // ---- A3: creators, in arrival order = candidate order
     for (int c = tid; c < cand_total; c += BEAM_THREADS) {
-      const Cand cd = cand[c];
+      const Cand cd = ua.cand[c];
       if (!(cd.score > JB200_LOG_ZERO)) continue;
       const unsigned seq = (unsigned)cd.src * SEQ_LOCAL + (unsigned)(c - offs[cd.src]);
-      if ((unsigned)__ldcg(slots.fs(cd.node)) == seq) atomicOr(bits + (c >> 5), 1u << (c & 31));
+      if ((unsigned)__ldcg(ua.slots.fs(cd.node)) == seq) atomicOr(ua.bits + (c >> 5), 1u << (c & 31));
     }
     __syncthreads();
     PROF_MARK(3);
-    int ncre_a;
-    {
-      int carry = 0;
-      for (int w0 = 0; w0 < nwords; w0 += BEAM_THREADS) {
-        const int w = w0 + tid;
-        const int cnt = (w < nwords) ? __popc(__ldcg(bits + w)) : 0;
-        int tot;
-        const int ex = block_excl_scan(cnt, s_warp, &tot);
-        if (w < nwords) wpre[w] = carry + ex;
-        carry += tot;
-      }
-      ncre_a = carry;
-    }
+    int ncre_a = rank_creators(ua.bits, ua.wpre, nwords, s_warp);
     if (ncre_a > MAXT) { if (tid == 0) s_overflow = 1; ncre_a = 0; }
     __syncthreads();
     PROF_MARK(4);
 
     // ---- A4: materialise the tokens of half A (no output probability yet) and mark their slots "exists"
     for (int c = tid; c < cand_total && ncre_a > 0; c += BEAM_THREADS) {
-      const unsigned wbits = __ldcg(bits + (c >> 5));
+      const unsigned wbits = __ldcg(ua.bits + (c >> 5));
       if (!((wbits >> (c & 31)) & 1u)) continue;
-      const int r = wpre[c >> 5] + __popc(wbits & ((1u << (c & 31)) - 1u));
-      const int node = cand[c].node;
-      const unsigned long long bk = __ldcg(slots.bk(node));
+      const int r = ua.wpre[c >> 5] + __popc(wbits & ((1u << (c & 31)) - 1u));
+      const int node = ua.cand[c].node;
+      const unsigned long long bk = __ldcg(ua.slots.bk(node));
       const unsigned seqw = ~(unsigned)(bk & 0xffffffffu);
       const int j = (int)(seqw >> SEQ_LOCAL_BITS), local = (int)(seqw & (SEQ_LOCAL - 1));
-      const Cand cd = cand[offs[j] + local];
+      const Cand cd = ua.cand[offs[j] + local];
       const Tok src = tl[ordl[j]];
       Tok nt; nt.node = node;
       nt.score = cd.score; nt.lscore = cd.lscore; nt.tre = src.tre; nt.cword = src.cword; nt.tre_wid = src.tre_wid;
       tn[r] = nt;
       heap[r + 1] = ((unsigned long long)(unsigned)r << 32) | __float_as_uint(nt.score);
-      slots.set(node, r - TOK_EXISTS, ((unsigned long long)fkey(nt.score) << 32) | 0xffffffffull);
+      ua.slots.set(node, r - TOK_EXISTS, ((unsigned long long)fkey(nt.score) << 32) | 0xffffffffull);
     }
     __syncthreads();
     PROF_MARK(5);
@@ -1374,7 +1761,7 @@ beam_kernel_mp(const BeamParams p) {
         ns_a = need;
         if (need < ncre_a - need) select_exact<true>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
         else select_exact<false>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
-        if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre_a, need, tn, heap, nullptr, &s_overflow);
+        if constexpr (CHECK) check_select(p.heap_chk + (size_t)u * (MAXT + 4), ncre_a, need, tn, heap, nullptr, &s_overflow);
       }
     }
     __syncthreads();
@@ -1399,16 +1786,11 @@ beam_kernel_mp(const BeamParams p) {
         const int ow = block_excl_scan(is_tr, s_warp, &tot_w);
         if (is_we) {
           const int ai = carry_a + oa;
-          if (ai < atom_cap && t > 0) {
-            jb200_atom a;
-            a.wid = nr.stend; a.backscore = tk.score;
-            a.begintime = (tk.tre < 0 ? -1 : araw[tk.tre].endtime) + 1;
-            a.endtime = t - 1; a.last = tk.tre; a.lscore = tk.lscore;
-            araw[ai] = a;
-          } else s_overflow = 1;
+          if (ai < ua.atom_cap && t > 0) ua.araw[ai] = trellis_atom(tk, nr.stend, t - 1, ua.araw);
+          else s_overflow = 1;
           if (is_tr) {
             const int wi = carry_w + ow;
-            if (wi < MAXW && ai < atom_cap) {
+            if (wi < MAXW && ai < ua.atom_cap) {
               WEnd w;
               const int sword = nr.stend;
               const int transp = p.is_transp[sword];
@@ -1416,7 +1798,7 @@ beam_kernel_mp(const BeamParams p) {
               w.base = tk.score;                                   // no wordend_a in multipath (beam.c:2307)
               w.transp2 = (transp && tk.cword >= 0 && p.is_transp[tk.cword]) ? 1 : 0;
               w.nintra = 0;
-              wend[wi] = w;
+              ua.wend[wi] = w;
               if (w.base > JB200_LOG_ZERO)
                 atomicMax(&s_webest, ((unsigned long long)fkey(w.base) << 32) | (unsigned)(~(unsigned)wi));
             } else s_overflow = 1;
@@ -1424,14 +1806,14 @@ beam_kernel_mp(const BeamParams p) {
         }
         carry_a += tot_a; carry_w += tot_w;
       }
-      if (tid == 0) { s_natoms = min(carry_a, atom_cap); s_E = min(carry_w, MAXW); }
+      if (tid == 0) { s_natoms = min(carry_a, ua.atom_cap); s_E = min(carry_w, MAXW); }
       nbits_b = carry_w * p.n_isoarc + p.n_sharc;
-      // carry_a > atom_cap: some word ends got no atom and no wend entry, and wend[0..E) would hold stale entries
-      if (carry_w > MAXW || nbits_b > p.maxbits || carry_a > atom_cap) { if (tid == 0) s_overflow = 1; nbits_b = 0; }
+      // carry_a > ua.atom_cap: some word ends got no atom and no ua.wend entry, and ua.wend[0..E) would hold stale entries
+      if (carry_w > MAXW || nbits_b > p.maxbits || carry_a > ua.atom_cap) { if (tid == 0) s_overflow = 1; nbits_b = 0; }
     }
     if (final) { n_left = ncre_a; __syncthreads(); break; }
     nwords = (nbits_b + 31) >> 5;
-    for (int w = tid; w < nwords; w += BEAM_THREADS) bits[w] = 0u;
+    for (int w = tid; w < nwords; w += BEAM_THREADS) ua.bits[w] = 0u;
     __syncthreads();
     PROF_MARK(1);
     const int E = (nbits_b > 0) ? s_E : 0;
@@ -1443,7 +1825,7 @@ beam_kernel_mp(const BeamParams p) {
       const float pa = __ldg(p.isoarc_a + ia);
       float best = JB200_LOG_ZERO, bestl = 0.0f; int beste = -1, firste = -1;
       for (int e = 0; e < E; e++) {
-        const WEnd w = wend[e];
+        const WEnd w = ua.wend[e];
         const float tmpprob = __ldg(p.iw + (size_t)w.last_word * p.n_iso + col);
         const float lsc = tmpprob * p.lm_weight + p.lm_penalty;
         float tmpsum = w.base;
@@ -1456,11 +1838,11 @@ beam_kernel_mp(const BeamParams p) {
         }
       }
       IsoCand ic; ic.score = best; ic.e = beste; ic.lscore = bestl; ic.first_e = firste;
-      iso[ia] = ic;
+      ua.iso[ia] = ic;
       if (firste >= 0) {
-        const unsigned sf = (unsigned)(wend[firste].j + 1) * SEQ_LOCAL + (unsigned)ia;
-        const unsigned sw = (unsigned)(wend[beste].j + 1) * SEQ_LOCAL + (unsigned)ia;
-        cand_atomics(slots, __ldg(p.isoarc_node + ia), best, sf, sw);
+        const unsigned sf = (unsigned)(ua.wend[firste].j + 1) * SEQ_LOCAL + (unsigned)ia;
+        const unsigned sw = (unsigned)(ua.wend[beste].j + 1) * SEQ_LOCAL + (unsigned)ia;
+        cand_atomics(ua.slots, __ldg(p.isoarc_node + ia), best, sf, sw);
       }
     }
     // ---- B3: best word end -> successors of the shared (1-gram factored) roots (beam.c:2549-2616)
@@ -1477,12 +1859,12 @@ beam_kernel_mp(const BeamParams p) {
       return v > JB200_LOG_ZERO;
     };
     if (have_we) {
-      wbest = wend[(unsigned)(~(unsigned)(webest & 0xffffffffu))];
+      wbest = ua.wend[(unsigned)(~(unsigned)(webest & 0xffffffffu))];
       for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
         float lsc, v;
         if (!shared_value(sa, lsc, v)) continue;
         const unsigned seq = (unsigned)(ns_a + 1) * SEQ_LOCAL + (unsigned)sa;
-        cand_atomics(slots, __ldg(p.sharc_node + sa), v, seq, seq);
+        cand_atomics(ua.slots, __ldg(p.sharc_node + sa), v, seq, seq);
       }
     }
     __syncthreads();
@@ -1490,38 +1872,26 @@ beam_kernel_mp(const BeamParams p) {
 
     // ---- B4: creators of half B (arrival order: word end major, then the factoring pass)
     for (int ia = tid; ia < p.n_isoarc; ia += BEAM_THREADS) {
-      const IsoCand ic = iso[ia];
+      const IsoCand ic = ua.iso[ia];
       if (ic.first_e < 0) continue;
-      const unsigned sf = (unsigned)(wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia;
-      if ((unsigned)__ldcg(slots.fs(__ldg(p.isoarc_node + ia))) == sf) {
+      const unsigned sf = (unsigned)(ua.wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia;
+      if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.isoarc_node + ia))) == sf) {
         const int pos = ic.first_e * p.n_isoarc + ia;
-        atomicOr(bits + (pos >> 5), 1u << (pos & 31));
+        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
       }
     }
     if (have_we) {
       for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
         const unsigned seq = (unsigned)(ns_a + 1) * SEQ_LOCAL + (unsigned)sa;
-        if ((unsigned)__ldcg(slots.fs(__ldg(p.sharc_node + sa))) == seq) {
+        if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.sharc_node + sa))) == seq) {
           const int pos = E * p.n_isoarc + sa;
-          atomicOr(bits + (pos >> 5), 1u << (pos & 31));
+          atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
         }
       }
     }
     __syncthreads();
     PROF_MARK(3);
-    int ncre;
-    {
-      int carry = 0;
-      for (int w0 = 0; w0 < nwords; w0 += BEAM_THREADS) {
-        const int w = w0 + tid;
-        const int cnt = (w < nwords) ? __popc(__ldcg(bits + w)) : 0;
-        int tot;
-        const int ex = block_excl_scan(cnt, s_warp, &tot);
-        if (w < nwords) wpre[w] = carry + ex;
-        carry += tot;
-      }
-      ncre = ncre_a + carry;
-    }
+    int ncre = ncre_a + rank_creators(ua.bits, ua.wpre, nwords, s_warp);
     if (ncre > MAXT) { if (tid == 0) s_overflow = 1; ncre = ncre_a; nbits_b = 0; }
     __syncthreads();
     PROF_MARK(4);
@@ -1533,24 +1903,24 @@ beam_kernel_mp(const BeamParams p) {
       if (j == ns_a + 1) {
         float lsc, v;
         shared_value(local, lsc, v);
-        nt.score = v; nt.lscore = lsc; nt.tre = wbest.atom; nt.cword = wbest.last_word; nt.tre_wid = araw[wbest.atom].wid;
+        nt.score = v; nt.lscore = lsc; nt.tre = wbest.atom; nt.cword = wbest.last_word; nt.tre_wid = ua.araw[wbest.atom].wid;
       } else {
-        const IsoCand ic = iso[local];
-        const WEnd w = wend[ic.e];
-        nt.score = ic.score; nt.lscore = ic.lscore; nt.tre = w.atom; nt.cword = w.last_word; nt.tre_wid = araw[w.atom].wid;
+        const IsoCand ic = ua.iso[local];
+        const WEnd w = ua.wend[ic.e];
+        nt.score = ic.score; nt.lscore = ic.lscore; nt.tre = w.atom; nt.cword = w.last_word; nt.tre_wid = ua.araw[w.atom].wid;
       }
     };
     auto settle = [&](int node, unsigned seq_first, unsigned seq_win, int pos) {
-      const int fs = __ldcg(slots.fs(node));
-      const unsigned seqw = ~(unsigned)(__ldcg(slots.bk(node)) & 0xffffffffu);
+      const int fs = __ldcg(ua.slots.fs(node));
+      const unsigned seqw = ~(unsigned)(__ldcg(ua.slots.bk(node)) & 0xffffffffu);
       if (fs < 0) {
         if (seqw != seq_win) return;
         Tok nt; nt.node = node;
         winner_content(seqw, nt);
         tn[fs + TOK_EXISTS] = nt;
       } else if ((unsigned)fs == seq_first) {
-        const unsigned wbits = __ldcg(bits + (pos >> 5));
-        const int r = ncre_a + wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
+        const unsigned wbits = __ldcg(ua.bits + (pos >> 5));
+        const int r = ncre_a + ua.wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
         Tok nt; nt.node = node;
         winner_content(seqw, nt);
         tn[r] = nt;
@@ -1558,10 +1928,10 @@ beam_kernel_mp(const BeamParams p) {
     };
     if (nbits_b > 0) {
       for (int ia = tid; ia < p.n_isoarc; ia += BEAM_THREADS) {
-        const IsoCand ic = iso[ia];
+        const IsoCand ic = ua.iso[ia];
         if (ic.first_e < 0) continue;
-        settle(__ldg(p.isoarc_node + ia), (unsigned)(wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia,
-               (unsigned)(wend[ic.e].j + 1) * SEQ_LOCAL + (unsigned)ia, ic.first_e * p.n_isoarc + ia);
+        settle(__ldg(p.isoarc_node + ia), (unsigned)(ua.wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia,
+               (unsigned)(ua.wend[ic.e].j + 1) * SEQ_LOCAL + (unsigned)ia, ic.first_e * p.n_isoarc + ia);
       }
       if (have_we)
         for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
@@ -1602,53 +1972,41 @@ beam_kernel_mp(const BeamParams p) {
       for (int k = tid; k < ns_new; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
     } else {
       // the input of select #2 cannot be rebuilt after the cut: the self-check keeps a copy
-      if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre, 0, nullptr, heap, nullptr, nullptr);
-      beam_cut(p, ca, ncre, s_hmaxkey, tn, slots, ordn, s_prof, s_tprev);
+      if constexpr (CHECK) check_select(p.heap_chk + (size_t)u * (MAXT + 4), ncre, 0, nullptr, heap, nullptr, nullptr);
+      beam_cut(p, ca, ncre, s_hmaxkey, tn, ua.slots, ordn, s_prof, s_tprev);
       slots_clean = true;
-      if (CHECK) check_select_mp(p.heap_chk + (size_t)u * (MAXT + 4), ncre, p.beam, nullptr, nullptr, ordn, &s_overflow);
+      if constexpr (CHECK) check_select(p.heap_chk + (size_t)u * (MAXT + 4), ncre, p.beam, nullptr, nullptr, ordn, &s_overflow);
     }
     PROF_MARK(6);
-    if (tid == 0) {
-      counts[2 * t] = ncre; counts[2 * t + 1] = ns_new;
-      s_ns = ns_new; s_cur = nxt;
-      if (p.prune_width >= 0.0f) {
-        const unsigned k = s_pmaxkey;
-        const unsigned b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
-        s_thr = __uint_as_float(b) - p.prune_width;
-      } else s_thr = JB200_LOG_ZERO;
-    }
+    // (s_pmaxkey starts at fkey(LOG_ZERO) here, never 0)
+    if (tid == 0) { end_frame(p, ua.counts, t, ncre, ns_new, s_pmaxkey, s_ns, s_thr); s_cur = nxt; }
     tnum_prev = ncre;
     __syncthreads();
     if (ncre == 0) { stopped = t; break; }      // beam.c:3012-3015
   }
 
   if (!ck_final) {
-    // more frames to come: park the scalar state (everything else already lives in the utterance's global work area)
-    if (tid == 0) {
-      ust->natoms = s_natoms; ust->overflow = s_overflow; ust->thr = s_thr; ust->ns = s_ns; ust->cur = s_cur;
-      ust->tnum_prev = tnum_prev; ust->stopped = stopped; ust->slots_clean = slots_clean ? 1 : 0; ust->n_left = 0;
-      ust->t_done = T;
-      long long _n = clock64(); s_prof[7] += _n - s_tprev;
-      for (int k = 0; k < 8; k++) ust->prof[k] = s_prof[k];
-      // the word ends of frame T-1 were stored in half B of that frame (end time T-2)
-      if (p.interim) interim_best(p, u, araw, (T >= 2 && stopped < 0) ? group0[T - 2] : s_natoms, s_natoms, T - 1);
-    }
+    if (tid == 0) park_scalars(p, u, ua, T, s_natoms, s_overflow, s_thr, s_ns, s_cur, tnum_prev, stopped, slots_clean, s_prof, s_tprev);
     return;
   }
   const int groups = (stopped >= 0) ? stopped : T;
 
   {
-    if (tid == 0 && T > 0) group0[groups] = s_natoms;
+    if (tid == 0 && T > 0) ua.group0[groups] = s_natoms;
     // leave the node slots clean for the next utterance that uses this work area
     // (only the unfinished final frame leaves any: every other frame's slots are reset by the next P0)
-    const Tok *tlast = tok0 + (size_t)(s_cur ^ 1) * MAXT;
-    for (int i = tid; i < n_left; i += BEAM_THREADS) {
-      const int node = tlast[i].node;
-      slots.reset(node);
-    }
+    SlotClear{ua.tok0 + (size_t)(s_cur ^ 1) * MAXT, n_left, ua.slots}.run(tid, BEAM_THREADS);
     __syncthreads();
   }
-  finalize_utt(p, u, tid, T, araw, newidx, group0, res, words, s_natoms, s_overflow, s_found, s_outbase, s_prof, s_tprev);
+  finalize_utt<false>(p, u, tid, T, ua.araw, ua.newidx, ua.group0, ua.res, ua.words, s_natoms, s_overflow, s_found, s_outbase, s_prof, s_tprev);
+}
+
+// the beam kernel for a tree (grammar mode runs on normal trees only); check: the JB200_CHECK_HEAP build
+using BeamKernel = void (*)(BeamParams);
+static BeamKernel beam_kernel_for(const bool grammar, const bool multipath, const bool check) {
+  if (multipath) return check ? beam_kernel_mp<true> : beam_kernel_mp<false>;
+  if (grammar) return check ? beam_kernel<true, true> : beam_kernel<true, false>;
+  return check ? beam_kernel<false, true> : beam_kernel<false, false>;
 }
 
 // ---- set-up kernels ------------------------------------------------------------------------------
@@ -1696,10 +2054,10 @@ struct jb200_decoder {
   std::vector<int> h_frame_off;
   float last_ms[4] = {0, 0, 0, 0};
   size_t smem_bytes = 0;
+  BeamKernel beam = nullptr;                    // beam_kernel_for the decoder's tree
   bool fetched = false;
   long long last_d2h = 0;
   int resident = 0;
-  bool grammar = false;
   // chunked launches: descriptors (a pinned staging copy and its device copy, one row of max_utts per chunk), parked state
   static constexpr int MAX_CHUNKS = 64;
   ChunkDesc *h_chunk = nullptr, *d_chunk = nullptr;
@@ -1727,23 +2085,21 @@ static void *arena_take(jb200_decoder *d, size_t bytes) {
   return p;
 }
 template <typename Tp>
-static int dev_upload(jb200_decoder *d, const Tp *src, size_t n, const Tp **dst) {
-  Tp *p = static_cast<Tp *>(arena_take(d, std::max<size_t>(n, 1) * sizeof(Tp)));
-  if (!p) {
-    JB_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(Tp)));
-    d->dev_allocs.push_back(p);
-  }
-  if (n) JB_CUDA(cudaMemcpy(p, src, n * sizeof(Tp), cudaMemcpyHostToDevice));
-  *dst = p;
-  return JB200_OK;
-}
-template <typename Tp>
 static int dev_alloc_shared(jb200_decoder *d, size_t n, Tp **dst) {
   Tp *p = static_cast<Tp *>(arena_take(d, std::max<size_t>(n, 1) * sizeof(Tp)));
   if (!p) {
     JB_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(Tp)));
     d->dev_allocs.push_back(p);
   }
+  *dst = p;
+  return JB200_OK;
+}
+template <typename Tp>
+static int dev_upload(jb200_decoder *d, const Tp *src, size_t n, const Tp **dst) {
+  Tp *p = nullptr;
+  const int rc = dev_alloc_shared(d, n, &p);
+  if (rc) return rc;
+  if (n) JB_CUDA(cudaMemcpy(p, src, n * sizeof(Tp), cudaMemcpyHostToDevice));
   *dst = p;
   return JB200_OK;
 }
@@ -2001,9 +2357,10 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
   // global-memory heap only: [7] replays on a shared-memory copy of the whole heap, [8] replays on the heap itself (top-and-tail copy)
   TRY(dev_alloc(d, 16, &P.misspec_counter));
   TRYC(cudaMemset(P.misspec_counter, 0, 16 * sizeof(unsigned long long)));
-  P.check_heap = getenv("JB200_CHECK_HEAP") ? atoi(getenv("JB200_CHECK_HEAP")) : 0;
+  // JB200_CHECK_HEAP=1: check every cut against the plain sequential replay
+  const bool check_heap = getenv("JB200_CHECK_HEAP") && atoi(getenv("JB200_CHECK_HEAP"));
   P.heap_chk = nullptr;
-  if (P.check_heap && P.multipath) TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_chk));
+  if (check_heap && P.multipath) TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_chk));
   P.lmc_bits = lmc_bits; P.lmc = nullptr;
   if (lmc_bits > 0) {
     TRY(dev_alloc_shared(d, (size_t)1 << lmc_bits, &P.lmc));
@@ -2056,8 +2413,8 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
     if (const char *e = getenv("JB200_PIPE_FRAMES")) d->pipe_frames = std::max(0, atoi(e));
   }
   d->smem_bytes = (heap_global ? (size_t)P.qcap * 8 + (size_t)(t->beam_width + 2) * 8 : (size_t)(maxt + 4) * 8) + offs_bytes;
-  d->grammar = grammar;
-  const void *kern = grammar ? (const void *)beam_kernel_grammar : P.multipath ? (P.check_heap ? (const void *)beam_kernel_mp<true> : (const void *)beam_kernel_mp<false>) : (const void *)beam_kernel;
+  d->beam = beam_kernel_for(grammar, P.multipath, check_heap);
+  const void *kern = (const void *)d->beam;
   TRYC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
   {
     int per_sm = 0, sms = 0;
@@ -2148,10 +2505,7 @@ static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index = 0, int in
   P.atoms_out_cap = d->atoms_cap; P.results = d->d_results; P.words = d->d_words; P.prof = d->d_prof;
   P.chunk = d->d_chunk + (size_t)chunk_index * d->max_utts; P.state = d->d_state;
   P.interim = interim; P.interim_words = d->d_interim_words; P.atoms_in_place = d->stream_mode ? 1 : 0;
-  if (d->grammar) beam_kernel_grammar<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
-  else if (P.multipath && P.check_heap) beam_kernel_mp<true><<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
-  else if (P.multipath) beam_kernel_mp<false><<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
-  else beam_kernel<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
+  d->beam<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
   JB_LAUNCH_CHECK();
   return JB200_OK;
 }
