@@ -103,6 +103,16 @@ def _f(a):
     return a.ctypes.data_as(D.F)
 
 
+def _utt_result(u, pa: int, pw: int) -> dict:
+    """one jb200_utt_result as a dict; its atoms and words are copied from the atom base pa and the word base pw"""
+    na, nw = int(u["n_atoms"]), int(u["n_words"])
+    atoms = np.ctypeslib.as_array(C.cast(pa + int(u["atom_offset"]) * ATOM_DT.itemsize, C.POINTER(C.c_uint8)),
+                                  shape=(max(na, 0) * ATOM_DT.itemsize,)).view(ATOM_DT).copy() if na > 0 else np.zeros(0, ATOM_DT)
+    words = np.ctypeslib.as_array(C.cast(pw + int(u["word_offset"]) * 4, D.I), shape=(nw,)).copy().tolist() if nw > 0 else []
+    return dict(status=int(u["status"]), n_frames=int(u["n_frames"]), atoms=atoms, words=words,
+                score=float(u["score"]), overflow=int(u["overflow"]))
+
+
 class GmmScorer:
     """All-state GMM scoring on the GPU (outprob_state/calc_mix/gprune_*/addlog_array/outprob_cd)."""
 
@@ -242,15 +252,7 @@ class Decoder:
         pu, pa, pw = self.raw_results()
         n = self._last_n if n_utts is None else n_utts
         utts = np.ctypeslib.as_array(C.cast(pu, C.POINTER(C.c_uint8)), shape=(n * UTT_DT.itemsize,)).view(UTT_DT)
-        out = []
-        for u in utts:
-            na, nw = int(u["n_atoms"]), int(u["n_words"])
-            atoms = np.ctypeslib.as_array(C.cast(pa + int(u["atom_offset"]) * ATOM_DT.itemsize, C.POINTER(C.c_uint8)),
-                                          shape=(max(na, 0) * ATOM_DT.itemsize,)).view(ATOM_DT).copy() if na > 0 else np.zeros(0, ATOM_DT)
-            words = np.ctypeslib.as_array(C.cast(pw + int(u["word_offset"]) * 4, D.I), shape=(nw,)).copy().tolist() if nw > 0 else []
-            out.append(dict(status=int(u["status"]), n_frames=int(u["n_frames"]), atoms=atoms, words=words,
-                            score=float(u["score"]), overflow=int(u["overflow"])))
-        return out
+        return [_utt_result(u, pa, pw) for u in utts]
 
     # the *_host entry points remember the batch size for results()
     _last_n = 0
@@ -303,12 +305,7 @@ class Decoder:
         pu, pa, pw = C.c_void_p(), C.c_void_p(), C.c_void_p()
         _check(lib().jb200_stream_result(self._h, stream, C.byref(pu), C.byref(pa), C.byref(pw)), "jb200_stream_result")
         u = np.ctypeslib.as_array(C.cast(pu.value, C.POINTER(C.c_uint8)), shape=(UTT_DT.itemsize,)).view(UTT_DT)[0]
-        na, nw = int(u["n_atoms"]), int(u["n_words"])
-        atoms = np.ctypeslib.as_array(C.cast(pa.value + int(u["atom_offset"]) * ATOM_DT.itemsize, C.POINTER(C.c_uint8)),
-                                      shape=(max(na, 0) * ATOM_DT.itemsize,)).view(ATOM_DT).copy() if na > 0 else np.zeros(0, ATOM_DT)
-        words = np.ctypeslib.as_array(C.cast(pw.value + int(u["word_offset"]) * 4, D.I), shape=(nw,)).copy().tolist() if nw > 0 else []
-        return dict(status=int(u["status"]), n_frames=int(u["n_frames"]), atoms=atoms, words=words,
-                    score=float(u["score"]), overflow=int(u["overflow"]))
+        return _utt_result(u, pa.value, pw.value)
 
     def handle_ptr(self):
         return self._h

@@ -89,6 +89,20 @@ struct UttState {
   long long prof[8];
 };
 
+// The beam-cut counters (BeamParams::cut_counters), summed over all frames since create
+enum CutCounter {
+  CUT_SEQ_FALLBACKS,     // fall-backs to the plain sequential replay: there are none, always 0
+  CUT_REPLAY_TICKS,      // replay ticks
+  CUT_REPLAY_EXTRACTS,   // extractions replayed
+  CUT_HELD_BACK,         // held-back starts of the replay (counted, not reported)
+  CUT_UPWARD,            // upward selects
+  CUT_CLOSED,            // of which closed form
+  CUT_RELOCATED,         // of which with relocations
+  CUT_GLOBAL_WHOLE,      // global-memory heap: replays on a shared-memory copy of the whole heap
+  CUT_GLOBAL_TOP_TAIL,   // global-memory heap: replays on the heap itself, its top and tail copied
+  CUT_SLOTS = 16         // slots allocated
+};
+
 struct BeamParams {
   // tree
   const NodeRec *nodes; const int *arc_to; const float *arc_a;
@@ -118,7 +132,7 @@ struct BeamParams {
   jb200_utt_result *results; int *words;
   long long *prof;            // [n_utts][8] cycle counters per phase, or NULL
   unsigned *bitmask; int *wordpre;   // per-utterance arrival-order bitmask [maxbits/32] and its word prefix counts
-  unsigned long long *misspec_counter;        // beam-cut counters, see jb200_decoder_create
+  unsigned long long *cut_counters;           // [CUT_SLOTS], indexed by CutCounter
   unsigned long long *lmc; int lmc_bits;      // memo of max_successor_prob, 2^lmc_bits entries (0 = off)
   int maxt, maxc, maxw, maxbits;
   // token sets too large for shared memory (wide beams on large trees): the heap-select array lives in global memory
@@ -537,8 +551,8 @@ __device__ void heap_extract_fast(const CutAreas &ca, const int n, const int ext
       unsigned ticks, stalls;
       heap_extract_pipe_warp6<MAXHEAP>(gcache, n, extract, lose_below, outv, lmaxt, threadIdx.x, ticks, stalls);
       if (threadIdx.x == 0) {
-        atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
-        atomicAdd(stats + 3, (unsigned long long)stalls); atomicAdd(stats + 7, 1ull);
+        atomicAdd(stats + CUT_REPLAY_TICKS, (unsigned long long)ticks); atomicAdd(stats + CUT_REPLAY_EXTRACTS, (unsigned long long)extract);
+        atomicAdd(stats + CUT_HELD_BACK, (unsigned long long)stalls); atomicAdd(stats + CUT_GLOBAL_WHOLE, 1ull);
       }
     }
     __syncthreads();
@@ -563,9 +577,9 @@ __device__ void heap_extract_fast(const CutAreas &ca, const int n, const int ext
     if (!__isShared(A)) heap_extract_pipe_global<MAXHEAP>(A, n, extract, lose_below, outv, maxt, hc, ticks, stalls);
     else heap_extract_pipe_warp6<MAXHEAP>(A, n, extract, lose_below, outv, maxt, threadIdx.x, ticks, stalls);
     if (threadIdx.x == 0) {
-      atomicAdd(stats + 1, (unsigned long long)ticks); atomicAdd(stats + 2, (unsigned long long)extract);
-      atomicAdd(stats + 3, (unsigned long long)stalls);
-      if (!__isShared(A)) atomicAdd(stats + 8, 1ull);
+      atomicAdd(stats + CUT_REPLAY_TICKS, (unsigned long long)ticks); atomicAdd(stats + CUT_REPLAY_EXTRACTS, (unsigned long long)extract);
+      atomicAdd(stats + CUT_HELD_BACK, (unsigned long long)stalls);
+      if (!__isShared(A)) atomicAdd(stats + CUT_GLOBAL_TOP_TAIL, 1ull);
     }
   }
   __syncthreads();
@@ -929,18 +943,22 @@ __device__ __forceinline__ void beam_cut(const BeamParams &p, const CutAreas &ca
     sc.run(tid, BEAM_THREADS);
     const int closed = heap_select_closed(heap, n, need, lose_below, maxt, ca.gq ? ca.gq : heap + n + 1, ca.gq ? p.sort_cap : maxt + 3 - n,
                                           reinterpret_cast<unsigned *>(ca.offs), 2 * (p.beam + 2), ordn, s_cf);
-    if (tid == 0) { atomicAdd(p.misspec_counter + 4, 1ull); if (closed) atomicAdd(p.misspec_counter + 5, 1ull); if (closed == 2) atomicAdd(p.misspec_counter + 6, 1ull); }
+    if (tid == 0) {
+      atomicAdd(p.cut_counters + CUT_UPWARD, 1ull);
+      if (closed) atomicAdd(p.cut_counters + CUT_CLOSED, 1ull);
+      if (closed == 2) atomicAdd(p.cut_counters + CUT_RELOCATED, 1ull);
+    }
     if (!closed) {
       heap_pad_sentinels<true>(heap, n, maxt);
       __syncthreads();
-      heap_extract_fast<true>(ca, n, need, lose_below, maxt, p.misspec_counter);
+      heap_extract_fast<true>(ca, n, need, lose_below, maxt, p.cut_counters);
       for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(outv[need - 1 - k] >> 32);
     }
   } else {
     // downward: no loser cut, no closed form; the idle warps reset the node slots during the replay
     heap_pad_sentinels<false>(heap, n, maxt);
     heap_build<false>(heap, n); PROF_MARK(7);
-    heap_extract_fast<false>(ca, n, n - need, -INFINITY, maxt, p.misspec_counter, &sc);
+    heap_extract_fast<false>(ca, n, n - need, -INFINITY, maxt, p.cut_counters, &sc);
     for (int k = tid; k < need; k += BEAM_THREADS) ordn[k] = (int)(heap[k + 1] >> 32);
   }
 }
@@ -1759,8 +1777,8 @@ beam_kernel_mp(const BeamParams p) {
         for (int k = tid; k < ns_a; k += BEAM_THREADS) ordn[k] = k;
       } else {
         ns_a = need;
-        if (need < ncre_a - need) select_exact<true>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
-        else select_exact<false>(ca, ncre_a, need, ordn, MAXT, p.misspec_counter);
+        if (need < ncre_a - need) select_exact<true>(ca, ncre_a, need, ordn, MAXT, p.cut_counters);
+        else select_exact<false>(ca, ncre_a, need, ordn, MAXT, p.cut_counters);
         if constexpr (CHECK) check_select(p.heap_chk + (size_t)u * (MAXT + 4), ncre_a, need, tn, heap, nullptr, &s_overflow);
       }
     }
@@ -2032,25 +2050,23 @@ using namespace jb200;
 struct jb200_decoder {
   jb200_gmm *am = nullptr;
   jb200_dnn *dnn = nullptr;
-  int device = 0, dim = 0, S = 0, row_stride = 0;
+  int device = 0, dim = 0, S = 0;
   int max_utts = 0, max_frames = 0;         // per batch: utterances, total frames
   int atoms_per_frame = 64;
+  // the one home of every device pointer fixed at create; launch_beam sets only the chunk row, interim and atoms_in_place
   BeamParams P{};
-  std::vector<void *> dev_allocs;
+  std::vector<void *> dev_allocs, host_allocs;  // device memory and pinned host memory, freed by jb200_decoder_destroy
   // read-only tables shared by all utterances (tree, LM, inter-word table, bigram memo) sit in ONE allocation
   char *arena = nullptr; size_t arena_size = 0, arena_used = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[5]{};
-  // batch buffers
+  // buffers the host writes and the kernel reads through P's const pointers
   float *d_feats = nullptr, *d_rows = nullptr;
   int *d_frame_off = nullptr; long long *d_atom_off = nullptr;
-  jb200_atom *d_atoms_out = nullptr; unsigned long long *d_atom_counter = nullptr;
-  jb200_utt_result *d_results = nullptr; int *d_words = nullptr; long long *d_prof = nullptr;
   // host results (pinned)
   jb200_utt_result *h_results = nullptr; jb200_atom *h_atoms = nullptr; int *h_words = nullptr;
   unsigned long long *h_counter = nullptr;
-  long long atoms_cap = 0;
-  int last_n = 0; long long last_atoms = 0; int last_total_frames = 0;
+  int last_n = 0, last_total_frames = 0;
   std::vector<int> h_frame_off;
   float last_ms[4] = {0, 0, 0, 0};
   size_t smem_bytes = 0;
@@ -2058,10 +2074,9 @@ struct jb200_decoder {
   bool fetched = false;
   long long last_d2h = 0;
   int resident = 0;
-  // chunked launches: descriptors (a pinned staging copy and its device copy, one row of max_utts per chunk), parked state
+  // chunked launches: descriptors (a pinned staging copy and its device copy, one row of max_utts per chunk)
   static constexpr int MAX_CHUNKS = 64;
   ChunkDesc *h_chunk = nullptr, *d_chunk = nullptr;
-  UttState *d_state = nullptr; int *d_interim_words = nullptr;
   // batch pipeline: scoring of time slice c+1 on its own stream beside the token passing of slice c
   cudaStream_t score_stream = nullptr;
   cudaEvent_t ev_slice[MAX_CHUNKS]{}; cudaEvent_t ev_score_begin = nullptr, ev_score_end = nullptr;
@@ -2085,25 +2100,6 @@ static void *arena_take(jb200_decoder *d, size_t bytes) {
   return p;
 }
 template <typename Tp>
-static int dev_alloc_shared(jb200_decoder *d, size_t n, Tp **dst) {
-  Tp *p = static_cast<Tp *>(arena_take(d, std::max<size_t>(n, 1) * sizeof(Tp)));
-  if (!p) {
-    JB_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(Tp)));
-    d->dev_allocs.push_back(p);
-  }
-  *dst = p;
-  return JB200_OK;
-}
-template <typename Tp>
-static int dev_upload(jb200_decoder *d, const Tp *src, size_t n, const Tp **dst) {
-  Tp *p = nullptr;
-  const int rc = dev_alloc_shared(d, n, &p);
-  if (rc) return rc;
-  if (n) JB_CUDA(cudaMemcpy(p, src, n * sizeof(Tp), cudaMemcpyHostToDevice));
-  *dst = p;
-  return JB200_OK;
-}
-template <typename Tp>
 static int dev_alloc(jb200_decoder *d, size_t n, Tp **dst) {
   Tp *p = nullptr;
   JB_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(Tp)));
@@ -2111,20 +2107,41 @@ static int dev_alloc(jb200_decoder *d, size_t n, Tp **dst) {
   *dst = p;
   return JB200_OK;
 }
+template <typename Tp>
+static int dev_alloc_shared(jb200_decoder *d, size_t n, Tp **dst) {
+  *dst = static_cast<Tp *>(arena_take(d, std::max<size_t>(n, 1) * sizeof(Tp)));
+  return *dst ? JB200_OK : dev_alloc(d, n, dst);
+}
+template <typename Tp>
+static int dev_upload(jb200_decoder *d, const Tp *src, size_t n, const Tp **dst) {
+  Tp *p = nullptr;
+  JB_RC(dev_alloc_shared(d, n, &p));
+  if (n) JB_CUDA(cudaMemcpy(p, src, n * sizeof(Tp), cudaMemcpyHostToDevice));
+  *dst = p;
+  return JB200_OK;
+}
+template <typename Tp>
+static int host_alloc(jb200_decoder *d, size_t n, Tp **dst) {
+  Tp *p = nullptr;
+  JB_CUDA(cudaMallocHost(&p, n * sizeof(Tp)));
+  d->host_allocs.push_back(p);
+  *dst = p;
+  return JB200_OK;
+}
+
+// resets the node slots of utterances [u0, u0 + n_utts) on the main stream
+static int reset_slots(jb200_decoder *d, int u0, int n_utts) {
+  const size_t tot = (size_t)n_utts * d->P.n_nodes;
+  fill_slots_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(d->P.slots + (size_t)u0 * d->P.n_nodes, tot);
+  JB_LAUNCH_CHECK();
+  return JB200_OK;
+}
 
 extern "C" void jb200_decoder_destroy(jb200_decoder *d) {
   if (!d) return;
   cudaSetDevice(d->device);
   for (void *p : d->dev_allocs) cudaFree(p);
-  if (d->h_results) cudaFreeHost(d->h_results);
-  if (d->h_atoms) cudaFreeHost(d->h_atoms);
-  if (d->h_words) cudaFreeHost(d->h_words);
-  if (d->h_counter) cudaFreeHost(d->h_counter);
-  if (d->h_chunk) cudaFreeHost(d->h_chunk);
-  if (d->h_seg) cudaFreeHost(d->h_seg);
-  if (d->h_aoff) cudaFreeHost(d->h_aoff);
-  if (d->h_state) cudaFreeHost(d->h_state);
-  if (d->h_interim_words) cudaFreeHost(d->h_interim_words);
+  for (void *p : d->host_allocs) cudaFreeHost(p);
   for (auto &e : d->ev) if (e) cudaEventDestroy(e);
   for (auto &e : d->ev_slice) if (e) cudaEventDestroy(e);
   if (d->ev_score_begin) cudaEventDestroy(d->ev_score_begin);
@@ -2134,8 +2151,25 @@ extern "C" void jb200_decoder_destroy(jb200_decoder *d) {
   delete d;
 }
 
-extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int max_utts, int max_frames, jb200_decoder **out) {
-  if (!t || !am || !out || max_utts < 1 || max_frames < 1) { set_error("jb200_decoder_create: bad argument"); return JB200_ERR_ARG; }
+// Multipath trees: the roots carry no output, so a cross-word transition into a root lands on the root's successors
+// (self, next, arcs: the order propagation visits them, beam.c:2467-2500).  The word-begin node of the head silence is
+// never entered (beam.c:2336-2342).  Calls f(list, root index, successor node, transition score) root-major, the isolated
+// roots (list 0) before the shared ones (list 1), in original node ids.
+template <typename F>
+static void for_root_successors(const jb200_tree_desc *t, F f) {
+  auto expand = [&](int list, int idx, int x) {
+    if (t->self_a[x] != JB200_LOG_ZERO) f(list, idx, x, t->self_a[x]);
+    if (t->next_a[x] != JB200_LOG_ZERO) f(list, idx, x + 1, t->next_a[x]);
+    for (int k = t->arc_off[x]; k < t->arc_off[x + 1]; k++) f(list, idx, t->arc_to[k], t->arc_a[k]);
+  };
+  const int head_begin = t->wordbegin[t->head_silwid];
+  for (int i = 0; i < t->n_iso; i++) if (t->iso_node[i] != head_begin) expand(0, i, t->iso_node[i]);
+  for (int i = 0; i < t->n_shared; i++) expand(1, i, t->shared_node[i]);
+}
+
+// The trees the beam kernels cannot decode.  Reads the descriptor alone; a count is checked before the loops that read
+// arrays of that size.
+static int check_tree(const jb200_tree_desc *t) {
   const bool grammar = (t->lm_type == JB200_LM_DFA);
   if (t->lm_type != JB200_LM_NGRAM && !grammar) { set_error("unknown language-model type %d", t->lm_type); return JB200_ERR_UNSUPPORTED; }
   if (grammar) {
@@ -2154,31 +2188,27 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
     set_error("the head silence word must exist and must not be transparent"); return JB200_ERR_UNSUPPORTED;
   }
   if (t->beam_width < 1 || t->beam_width > 8000) { set_error("beam width %d outside 1..8000", t->beam_width); return JB200_ERR_UNSUPPORTED; }
-  jb200_decoder *d = new jb200_decoder();
-  d->am = am; d->device = gmm_device(am); d->dim = gmm_dim(am);
-  d->S = jb200_gmm_n_states(am);
-  d->row_stride = (d->S + 3) & ~3;
-  d->max_utts = max_utts; d->max_frames = max_frames;
-  if (const char *e = getenv("JB200_ATOMS_PER_FRAME")) d->atoms_per_frame = std::max(4, atoi(e));
-  int rc;
-#define TRY(x) do { rc = (x); if (rc) { jb200_decoder_destroy(d); return rc; } } while (0)
-#define TRYC(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error("%s: %s", #x, cudaGetErrorString(_e)); jb200_decoder_destroy(d); return JB200_ERR_CUDA; } } while (0)
-  TRYC(cudaSetDevice(d->device));
-  TRYC(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-  for (auto &e : d->ev) TRYC(cudaEventCreate(&e));
-
-  BeamParams &P = d->P;
-  const int n = t->n_nodes;
-  // bigram-factoring memo, 2^21 entries: keys are (word id, successor slot) packed 16+16, so it needs both below 65535
-  const int lmc_bits = (t->n_words >= 65535 || t->n_scword >= 65535) ? 0 : 21;
-  {
-    // shared read-only tables: nodes 32 B, arcs 8 B, context table, inter-word table, bigram memo, LM arrays (+ slack)
-    size_t est = (size_t)n * 32 + (size_t)t->n_arcs * 8 * 3 + (size_t)t->n_rset * (t->n_ctx + 1) * 4 + (size_t)t->n_words * 32 +
-                 (size_t)t->n_words * std::max(t->n_iso, 1) * (grammar ? 1 : 4) + ((size_t)8 << lmc_bits) +
-                 (size_t)t->lm_nvocab * 16 + (size_t)t->lm_nbigram * 8 + (size_t)(t->n_iso + t->n_shared + t->n_fscore + t->n_scword) * 16 + (4u << 20);
-    if (cudaMalloc(&d->arena, est) == cudaSuccess) { d->arena_size = est; d->dev_allocs.push_back(d->arena); }
-    else { d->arena = nullptr; cudaGetLastError(); }
+  for (int o = 0; o < t->n_nodes; o++) {
+    const int style = t->outstyle[o];
+    if (style > 3 && !(style == 255 && t->multipath)) { set_error("non-emitting node in a non-multipath tree"); return JB200_ERR_UNSUPPORTED; }
   }
+  for (int i = 0; i < t->n_shared; i++)
+    if (t->scid[t->shared_node[i]] >= 0) { set_error("shared root without 1-gram factoring value"); return JB200_ERR_ARG; }
+  // a root, or on a multipath tree a root's successor, is numbered in the low SEQ_LOCAL_BITS of an arrival sequence number
+  long long n_arcs[2] = {0, 0};
+  if (t->multipath) for_root_successors(t, [&](int list, int, int, float) { n_arcs[list]++; });
+  if (t->n_iso + 1024 >= (int)SEQ_LOCAL || n_arcs[0] >= SEQ_LOCAL || n_arcs[1] >= SEQ_LOCAL || t->n_shared >= (int)SEQ_LOCAL) {
+    set_error("too many tree roots (%d isolated, %d shared) for the arrival-order numbering", t->n_iso, t->n_shared);
+    return JB200_ERR_UNSUPPORTED;
+  }
+  return JB200_OK;
+}
+
+// Create, step 1: the tree, renumbered, and its tables
+static int upload_tree(jb200_decoder *d, const jb200_tree_desc *t) {
+  BeamParams &P = d->P;
+  const bool grammar = (t->lm_type == JB200_LM_DFA);
+  const int n = t->n_nodes;
   // Node numbering.  The host numbers the nodes word by word (a word's own nodes are consecutive), so the ~2400 nodes a
   // frame touches are spread over the whole tree although 85 % of them sit in its first three levels (half of a frame's
   // tokens are the roots that a word end fans out to): one 128-byte line of per-node arrival slots per token.  Node ids
@@ -2216,223 +2246,252 @@ extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int
       for (int k = t->arc_off[o]; k < t->arc_off[o + 1]; k++) { arc_to_n[ao] = perm[t->arc_to[k]]; arc_a_n[ao] = t->arc_a[k]; ao++; }
       r.stend = t->stend[o]; r.scid = t->scid[o];
       const int style = t->outstyle[o];
-      if (style > 3 && !(style == 255 && t->multipath)) { set_error("non-emitting node in a non-multipath tree"); jb200_decoder_destroy(d); return JB200_ERR_UNSUPPORTED; }
       r.out = (style == 255) ? (int)0xF0000000u : (int)(((unsigned)style << 28) | (unsigned)(t->out_ref[o] & 0x0fffffff));
       r.next = (r.next_a != JB200_LOG_ZERO && o + 1 < n) ? perm[o + 1] : i;
     }
   }
-  TRY(dev_upload(d, nodes.data(), nodes.size(), &P.nodes));
-  TRY(dev_upload(d, arc_to_n.data(), (size_t)t->n_arcs, &P.arc_to));
-  TRY(dev_upload(d, arc_a_n.data(), (size_t)t->n_arcs, &P.arc_a));
-  TRY(dev_upload(d, t->rset_ctx, (size_t)t->n_rset * (t->n_ctx + 1), &P.rset_ctx));
-  TRY(dev_upload(d, t->word_ctx, (size_t)t->n_words, &P.word_ctx));
+  JB_RC(dev_upload(d, nodes.data(), nodes.size(), &P.nodes));
+  JB_RC(dev_upload(d, arc_to_n.data(), (size_t)t->n_arcs, &P.arc_to));
+  JB_RC(dev_upload(d, arc_a_n.data(), (size_t)t->n_arcs, &P.arc_a));
+  JB_RC(dev_upload(d, t->rset_ctx, (size_t)t->n_rset * (t->n_ctx + 1), &P.rset_ctx));
+  JB_RC(dev_upload(d, t->word_ctx, (size_t)t->n_words, &P.word_ctx));
   P.n_ctx = t->n_ctx;
-  { const std::vector<int> v = remap(t->iso_node, (size_t)t->n_iso); TRY(dev_upload(d, v.data(), v.size(), &P.iso_node)); }
-  TRY(dev_upload(d, t->iso_id, (size_t)t->n_iso, &P.iso_id));
+  { const std::vector<int> v = remap(t->iso_node, (size_t)t->n_iso); JB_RC(dev_upload(d, v.data(), v.size(), &P.iso_node)); }
+  JB_RC(dev_upload(d, t->iso_id, (size_t)t->n_iso, &P.iso_id));
   P.n_iso = t->n_iso;
-  { const std::vector<int> v = remap(t->shared_node, (size_t)t->n_shared); TRY(dev_upload(d, v.data(), v.size(), &P.shared_node)); }
+  { const std::vector<int> v = remap(t->shared_node, (size_t)t->n_shared); JB_RC(dev_upload(d, v.data(), v.size(), &P.shared_node)); }
   {
+    // check_tree: every shared root has a 1-gram factoring value
     std::vector<float> sf(std::max(t->n_shared, 1));
-    for (int i = 0; i < t->n_shared; i++) {
-      const int sc = t->scid[t->shared_node[i]];
-      if (sc >= 0) { set_error("shared root without 1-gram factoring value"); jb200_decoder_destroy(d); return JB200_ERR_ARG; }
-      sf[i] = t->fscore[-sc];
-    }
-    TRY(dev_upload(d, sf.data(), (size_t)t->n_shared, &P.shared_f));
+    for (int i = 0; i < t->n_shared; i++) sf[i] = t->fscore[-t->scid[t->shared_node[i]]];
+    JB_RC(dev_upload(d, sf.data(), (size_t)t->n_shared, &P.shared_f));
   }
   P.n_shared = t->n_shared;
   P.multipath = t->multipath ? 1 : 0;
-  P.cp_allowed = nullptr; P.init_node = nullptr; P.init_lscore = nullptr; P.n_init = 0; P.penalty1 = 0.0f;
+  P.head_node = grammar ? 0 : perm[t->wordbegin[t->head_silwid]]; P.n_nodes = n;
   if (grammar) {
-    TRY(dev_upload(d, t->cp_allowed, (size_t)t->n_words * t->n_iso, &P.cp_allowed));
-    { const std::vector<int> v = remap(t->init_node, (size_t)t->n_init); TRY(dev_upload(d, v.data(), v.size(), &P.init_node)); }
-    TRY(dev_upload(d, t->init_lscore, (size_t)t->n_init, &P.init_lscore));
+    JB_RC(dev_upload(d, t->cp_allowed, (size_t)t->n_words * t->n_iso, &P.cp_allowed));
+    { const std::vector<int> v = remap(t->init_node, (size_t)t->n_init); JB_RC(dev_upload(d, v.data(), v.size(), &P.init_node)); }
+    JB_RC(dev_upload(d, t->init_lscore, (size_t)t->n_init, &P.init_lscore));
     P.n_init = t->n_init; P.penalty1 = t->penalty1;
   }
-  {
-    // multipath: expand the roots into their successors (self, next, arcs: the order propagation visits them,
-    // beam.c:2467-2500); the word-begin node of the head silence is never entered (beam.c:2336-2342)
-    std::vector<int> ia_node, ia_iso, sa_node, sa_sh; std::vector<float> ia_a, sa_a;
-    if (t->multipath) {
-      auto expand = [&](int root, int idx, std::vector<int> &vn, std::vector<int> &vi, std::vector<float> &va) {
-        if (t->self_a[root] != JB200_LOG_ZERO) { vn.push_back(perm[root]); vi.push_back(idx); va.push_back(t->self_a[root]); }
-        if (t->next_a[root] != JB200_LOG_ZERO) { vn.push_back(perm[root + 1]); vi.push_back(idx); va.push_back(t->next_a[root]); }
-        for (int k = t->arc_off[root]; k < t->arc_off[root + 1]; k++) { vn.push_back(perm[t->arc_to[k]]); vi.push_back(idx); va.push_back(t->arc_a[k]); }
-      };
-      const int head_begin = t->wordbegin[t->head_silwid];
-      for (int i = 0; i < t->n_iso; i++) if (t->iso_node[i] != head_begin) expand(t->iso_node[i], i, ia_node, ia_iso, ia_a);
-      for (int i = 0; i < t->n_shared; i++) expand(t->shared_node[i], i, sa_node, sa_sh, sa_a);
-    }
-    P.n_isoarc = (int)ia_node.size(); P.n_sharc = (int)sa_node.size();
-    TRY(dev_upload(d, ia_node.data(), ia_node.size(), &P.isoarc_node));
-    TRY(dev_upload(d, ia_iso.data(), ia_iso.size(), &P.isoarc_iso));
-    TRY(dev_upload(d, ia_a.data(), ia_a.size(), &P.isoarc_a));
-    TRY(dev_upload(d, sa_node.data(), sa_node.size(), &P.sharc_node));
-    TRY(dev_upload(d, sa_sh.data(), sa_sh.size(), &P.sharc_shared));
-    TRY(dev_upload(d, sa_a.data(), sa_a.size(), &P.sharc_a));
-    if (t->n_iso + 1024 >= (int)SEQ_LOCAL || P.n_isoarc >= (int)SEQ_LOCAL || P.n_sharc >= (int)SEQ_LOCAL || t->n_shared >= (int)SEQ_LOCAL) {
-      set_error("too many tree roots (%d isolated, %d shared) for the arrival-order numbering", t->n_iso, t->n_shared);
-      jb200_decoder_destroy(d); return JB200_ERR_UNSUPPORTED;
-    }
-  }
-  TRY(dev_upload(d, t->wordend_a, (size_t)t->n_words, &P.wordend_a));
-  TRY(dev_upload(d, t->is_transparent, (size_t)t->n_words, &P.is_transp));
-  TRY(dev_upload(d, t->wton, (size_t)t->n_words, &P.wton));
-  TRY(dev_upload(d, t->cprob, (size_t)t->n_words, &P.cprob));
-  TRY(dev_upload(d, t->fscore, (size_t)t->n_fscore, &P.fscore));
-  TRY(dev_upload(d, t->scword, (size_t)t->n_scword, &P.scword));
-  TRY(dev_upload(d, t->uni_prob, (size_t)t->lm_nvocab, &P.uni_prob));
-  TRY(dev_upload(d, t->uni_bow, (size_t)t->lm_nvocab, &P.uni_bow));
-  TRY(dev_upload(d, t->bi_bgn, (size_t)t->lm_nvocab, &P.bi_bgn));
-  TRY(dev_upload(d, t->bi_num, (size_t)t->lm_nvocab, &P.bi_num));
-  TRY(dev_upload(d, t->bi_wid, (size_t)t->lm_nbigram, &P.bi_wid));
-  TRY(dev_upload(d, t->bi_prob, (size_t)t->lm_nbigram, &P.bi_prob));
+  // multipath: the successors of the isolated roots (list 0) and of the shared roots (list 1)
+  std::vector<int> rs_node[2], rs_root[2]; std::vector<float> rs_a[2];
+  if (t->multipath)
+    for_root_successors(t, [&](int list, int idx, int x, float a) { rs_node[list].push_back(perm[x]); rs_root[list].push_back(idx); rs_a[list].push_back(a); });
+  P.n_isoarc = (int)rs_node[0].size(); P.n_sharc = (int)rs_node[1].size();
+  JB_RC(dev_upload(d, rs_node[0].data(), rs_node[0].size(), &P.isoarc_node));
+  JB_RC(dev_upload(d, rs_root[0].data(), rs_root[0].size(), &P.isoarc_iso));
+  JB_RC(dev_upload(d, rs_a[0].data(), rs_a[0].size(), &P.isoarc_a));
+  JB_RC(dev_upload(d, rs_node[1].data(), rs_node[1].size(), &P.sharc_node));
+  JB_RC(dev_upload(d, rs_root[1].data(), rs_root[1].size(), &P.sharc_shared));
+  JB_RC(dev_upload(d, rs_a[1].data(), rs_a[1].size(), &P.sharc_a));
+  return JB200_OK;
+}
+
+// Create, step 2: the LM tables and the inter-word table
+static int upload_lm(jb200_decoder *d, const jb200_tree_desc *t) {
+  BeamParams &P = d->P;
+  const bool grammar = (t->lm_type == JB200_LM_DFA);
+  JB_RC(dev_upload(d, t->wordend_a, (size_t)t->n_words, &P.wordend_a));
+  JB_RC(dev_upload(d, t->is_transparent, (size_t)t->n_words, &P.is_transp));
+  JB_RC(dev_upload(d, t->wton, (size_t)t->n_words, &P.wton));
+  JB_RC(dev_upload(d, t->cprob, (size_t)t->n_words, &P.cprob));
+  JB_RC(dev_upload(d, t->fscore, (size_t)t->n_fscore, &P.fscore));
+  JB_RC(dev_upload(d, t->scword, (size_t)t->n_scword, &P.scword));
+  JB_RC(dev_upload(d, t->uni_prob, (size_t)t->lm_nvocab, &P.uni_prob));
+  JB_RC(dev_upload(d, t->uni_bow, (size_t)t->lm_nvocab, &P.uni_bow));
+  JB_RC(dev_upload(d, t->bi_bgn, (size_t)t->lm_nvocab, &P.bi_bgn));
+  JB_RC(dev_upload(d, t->bi_num, (size_t)t->lm_nvocab, &P.bi_num));
+  JB_RC(dev_upload(d, t->bi_wid, (size_t)t->lm_nbigram, &P.bi_wid));
+  JB_RC(dev_upload(d, t->bi_prob, (size_t)t->lm_nbigram, &P.bi_prob));
   P.lm_mode = t->lm_mode; P.lm_unk_id = t->lm_unk_id; P.lm_unk_num_log = t->lm_unk_num_log;
   P.lm_weight = t->lm_weight; P.lm_penalty = t->lm_penalty; P.lm_penalty_trans = t->lm_penalty_trans;
   P.prune_width = t->score_pruning_width;
-  P.head_node = grammar ? 0 : perm[t->wordbegin[t->head_silwid]]; P.tail_silwid = t->tail_silwid; P.beam = t->beam_width; P.n_nodes = n;
+  P.tail_silwid = t->tail_silwid; P.beam = t->beam_width;
   // cd sets come from the AM handle's descriptor: re-upload from the gmm handle is not exposed, so the
   // decoder asks the scorer for its device copies
-  {
-    const int *co = nullptr, *cs = nullptr; int meth = 0, nb = 0;
-    gmm_cd_device(am, &co, &cs, &meth, &nb);
-    P.cd_off = co; P.cd_states = cs; P.iwcd_method = meth; P.iwcd_nbest = nb;
-  }
+  gmm_cd_device(d->am, &P.cd_off, &P.cd_states, &P.iwcd_method, &P.iwcd_nbest);
   // inter-word bigram rows for every last word (the reference's iw_sc_cache, fully populated)
-  {
-    const int *d_iso_word = nullptr;
-    TRY(dev_upload(d, t->iso_word, (size_t)t->n_iso, &d_iso_word));
-    float *iw = nullptr;
-    TRY(dev_alloc_shared(d, (size_t)t->n_words * std::max(t->n_iso, 1), &iw));
-    P.iw = iw;
-    const long long tot = grammar ? 0 : (long long)t->n_words * t->n_iso;     // grammar mode reads cp_allowed instead
-    if (tot > 0) {
-      iw_table_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(P, d_iso_word, iw, t->n_words);
-      g_launches.fetch_add(1);
-      TRYC(cudaGetLastError());
-    }
+  const int *d_iso_word = nullptr;
+  JB_RC(dev_upload(d, t->iso_word, (size_t)t->n_iso, &d_iso_word));
+  float *iw = nullptr;
+  JB_RC(dev_alloc_shared(d, (size_t)t->n_words * std::max(t->n_iso, 1), &iw));
+  P.iw = iw;
+  const long long tot = grammar ? 0 : (long long)t->n_words * t->n_iso;     // grammar mode reads cp_allowed instead
+  if (tot > 0) {
+    iw_table_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(P, d_iso_word, iw, t->n_words);
+    JB_LAUNCH_CHECK();
   }
-  // work areas
+  return JB200_OK;
+}
+
+// Create, step 3: the sizes of the beam cut, from the beam width, the number of start tokens and the device's opt-in
+// shared memory per block.  tests/test_gpu_beam_widths.py restates the heap placement rule.
+// maxt: token capacity of a frame; sort_cap, qcap: see BeamParams (global heap only); smem_bytes: the kernel's dynamic share
+struct CutSizing { int maxt; bool heap_global; int sort_cap, qcap; size_t smem_bytes; };
+static int size_cut(int beam, int n_start, int smem_optin, CutSizing *cs) {
   // the reference starts at 2*beam+startnum tokens and grows on demand; we size once and flag overflow.  Seen on the
   // 20k-word tree: 4.6*beam at -b 800 (of which startnum = 1375 root tokens), 4.7*beam at -b 4000.  The array lives
   // in shared memory, and what it takes is lost to L1 (5*beam+startnum at -b 800 costs 30 % of the kernel's speed).
-  int maxt = (std::max(4 * t->beam_width + t->n_start, 5 * t->beam_width) + 64 + 3) & ~3;
+  int maxt = (std::max(4 * beam + n_start, 5 * beam) + 64 + 3) & ~3;
   // Where the heap-select array lives.  Shared memory as long as one block's share fits; a wide beam on a large tree
   // (-b 4000 on the 60k-word multipath tree creates up to 8.5 x beam tokens a frame) goes to global memory instead,
   // with room for 9 x beam + startnum tokens, and shared memory keeps only the closed form's sort area.
-  const size_t offs_bytes = (size_t)(t->beam_width + 2) * 4 * 2;
-  int smem_limit = 0;
-  TRYC(cudaDeviceGetAttribute(&smem_limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->device));
-  smem_limit -= 2048;                                       // static shared variables of the kernels
+  const size_t offs_bytes = (size_t)(beam + 2) * 4 * 2;
+  const int smem_limit = smem_optin - 2048;                 // static shared variables of the kernels
   const bool heap_global = (size_t)(maxt + 4) * 8 + offs_bytes > (size_t)smem_limit / 2;   // would leave one block per SM
-  P.heap_g = nullptr; P.sort_cap = 0; P.qcap = 0;
+  int sort_cap = 0, qcap = 0;
   if (heap_global) {
-    maxt = std::min(65000, (std::max(maxt, 9 * t->beam_width + t->n_start) + 3) & ~3);
-    int sc = 1024; while (sc < 2 * t->beam_width && sc < 16384) sc <<= 1;       // candidates = beam + one histogram bin
-    const size_t tail_bytes = (size_t)(t->beam_width + 2) * 8;                   // the replay's copy of the tail slots
-    if ((size_t)sc * 8 + offs_bytes + tail_bytes > (size_t)smem_limit) { set_error("beam width %d needs more shared memory than the device has", t->beam_width); jb200_decoder_destroy(d); return JB200_ERR_UNSUPPORTED; }
-    P.sort_cap = sc;
+    maxt = std::min(65000, (std::max(maxt, 9 * beam + n_start) + 3) & ~3);
+    sort_cap = 1024; while (sort_cap < 2 * beam && sort_cap < 16384) sort_cap <<= 1;   // candidates = beam + one histogram bin
+    const size_t tail_bytes = (size_t)(beam + 2) * 8;                                 // the replay's copy of the tail slots
+    if ((size_t)sort_cap * 8 + offs_bytes + tail_bytes > (size_t)smem_limit) { set_error("beam width %d needs more shared memory than the device has", beam); return JB200_ERR_UNSUPPORTED; }
     // what is left of shared memory holds the top levels of the heap during a replay (one block per SM: the replay is all
     // that matters at these beam widths)
-    int qc = sc;
-    while ((size_t)qc * 2 * 8 + offs_bytes + tail_bytes <= (size_t)smem_limit && qc * 2 <= ((maxt + 4) | 1023) + 1) qc <<= 1;
-    P.qcap = qc;
-    TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_g));
+    qcap = sort_cap;
+    while ((size_t)qcap * 2 * 8 + offs_bytes + tail_bytes <= (size_t)smem_limit && qcap * 2 <= ((maxt + 4) | 1023) + 1) qcap <<= 1;
   }
+  const size_t heap_bytes = heap_global ? (size_t)qcap * 8 + (size_t)(beam + 2) * 8 : (size_t)(maxt + 4) * 8;
+  *cs = CutSizing{maxt, heap_global, sort_cap, qcap, heap_bytes + offs_bytes};
+  return JB200_OK;
+}
+
+// Create, step 4: the per-utterance work areas, the batch buffers, the pipeline's stream and events, the kernel set-up
+static int alloc_work(jb200_decoder *d, const jb200_tree_desc *t, const CutSizing &cs) {
+  BeamParams &P = d->P;
+  const int mu = d->max_utts, mf = d->max_frames, maxt = cs.maxt, MC = jb200_decoder::MAX_CHUNKS;
+  P.sort_cap = cs.sort_cap; P.qcap = cs.qcap;
+  if (cs.heap_global) JB_RC(dev_alloc(d, (size_t)mu * (maxt + 4), &P.heap_g));
   P.maxt = maxt; P.maxc = 4 * maxt; P.maxw = t->beam_width + 1;
-  TRY(dev_alloc(d, (size_t)max_utts * 2 * maxt, &P.tok));
-  TRY(dev_alloc(d, (size_t)max_utts * 2 * maxt, &P.order));
-  TRY(dev_alloc(d, (size_t)max_utts * n, &P.slots));
-  TRY(dev_alloc(d, (size_t)max_utts * P.maxc, &P.cand));
-  TRY(dev_alloc(d, (size_t)max_utts * P.maxc, &P.candb));
-  TRY(dev_alloc(d, (size_t)max_utts * (t->beam_width + 2), &P.surv));
+  JB_RC(dev_alloc(d, (size_t)mu * 2 * maxt, &P.tok));
+  JB_RC(dev_alloc(d, (size_t)mu * 2 * maxt, &P.order));
+  JB_RC(dev_alloc(d, (size_t)mu * P.n_nodes, &P.slots));
+  JB_RC(dev_alloc(d, (size_t)mu * P.maxc, &P.cand));
+  JB_RC(dev_alloc(d, (size_t)mu * P.maxc, &P.candb));
+  JB_RC(dev_alloc(d, (size_t)mu * (t->beam_width + 2), &P.surv));
   const int n_isoent = std::max(std::max(t->n_iso, P.n_isoarc), 1);
-  TRY(dev_alloc(d, (size_t)max_utts * n_isoent, &P.iso));
-  TRY(dev_alloc(d, (size_t)max_utts * P.maxw, &P.wend));
+  JB_RC(dev_alloc(d, (size_t)mu * n_isoent, &P.iso));
+  JB_RC(dev_alloc(d, (size_t)mu * P.maxw, &P.wend));
   P.maxbits = (P.maxc + std::min(P.maxw, 256) * n_isoent + std::max(t->n_shared, P.n_sharc) + 63) & ~31;
-  TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.bitmask));
-  TRY(dev_alloc(d, (size_t)max_utts * (P.maxbits >> 5), &P.wordpre));
-  // beam-cut counters: [0] fall-backs to the plain sequential replay (there are none: always 0), [1] replay ticks,
-  // [2] extractions replayed, [3] held-back starts, [4] upward selects, [5] of which closed form, [6] of which with relocations,
-  // global-memory heap only: [7] replays on a shared-memory copy of the whole heap, [8] replays on the heap itself (top-and-tail copy)
-  TRY(dev_alloc(d, 16, &P.misspec_counter));
-  TRYC(cudaMemset(P.misspec_counter, 0, 16 * sizeof(unsigned long long)));
+  JB_RC(dev_alloc(d, (size_t)mu * (P.maxbits >> 5), &P.bitmask));
+  JB_RC(dev_alloc(d, (size_t)mu * (P.maxbits >> 5), &P.wordpre));
+  JB_RC(dev_alloc(d, CUT_SLOTS, &P.cut_counters));
+  JB_CUDA(cudaMemset(P.cut_counters, 0, CUT_SLOTS * sizeof(unsigned long long)));
   // JB200_CHECK_HEAP=1: check every cut against the plain sequential replay
   const bool check_heap = getenv("JB200_CHECK_HEAP") && atoi(getenv("JB200_CHECK_HEAP"));
-  P.heap_chk = nullptr;
-  if (check_heap && P.multipath) TRY(dev_alloc(d, (size_t)max_utts * (maxt + 4), &P.heap_chk));
-  P.lmc_bits = lmc_bits; P.lmc = nullptr;
-  if (lmc_bits > 0) {
-    TRY(dev_alloc_shared(d, (size_t)1 << lmc_bits, &P.lmc));
-    TRYC(cudaMemsetAsync(P.lmc, 0xff, sizeof(unsigned long long) << lmc_bits, d->stream));
+  if (check_heap && P.multipath) JB_RC(dev_alloc(d, (size_t)mu * (maxt + 4), &P.heap_chk));
+  if (P.lmc_bits > 0) {
+    JB_RC(dev_alloc_shared(d, (size_t)1 << P.lmc_bits, &P.lmc));
+    JB_CUDA(cudaMemsetAsync(P.lmc, 0xff, sizeof(unsigned long long) << P.lmc_bits, d->stream));
   }
-  P.chunk = nullptr; P.state = nullptr; P.interim = 0; P.interim_words = nullptr; P.atoms_in_place = 0;
-  {
-    size_t tot = (size_t)max_utts * n;
-    fill_slots_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(P.slots, tot);
-    g_launches.fetch_add(1);
-    TRYC(cudaGetLastError());
-  }
-  d->atoms_cap = (long long)max_frames * d->atoms_per_frame + (long long)max_utts * 64;
-  TRY(dev_alloc(d, (size_t)d->atoms_cap, &P.atoms_raw));
-  TRY(dev_alloc(d, (size_t)d->atoms_cap, &P.newidx));
-  TRY(dev_alloc(d, (size_t)max_frames + max_utts + 8, &P.group0));
-  TRY(dev_alloc(d, (size_t)max_frames * 2 + 8, &P.counts));
-  TRY(dev_alloc(d, (size_t)d->atoms_cap, &d->d_atoms_out));
-  TRY(dev_alloc(d, 1, &d->d_atom_counter));
-  TRY(dev_alloc(d, (size_t)max_utts, &d->d_results));
-  TRY(dev_alloc(d, (size_t)max_utts * MAX_WORDS, &d->d_words));
-  TRY(dev_alloc(d, (size_t)max_utts * 8, &d->d_prof));
-  TRY(dev_alloc(d, (size_t)max_utts + 1, &d->d_frame_off));
-  TRY(dev_alloc(d, (size_t)max_utts + 1, &d->d_atom_off));
-  TRY(dev_alloc(d, (size_t)max_frames * d->dim, &d->d_feats));
-  TRY(dev_alloc(d, (size_t)max_frames * d->row_stride, &d->d_rows));
-  TRYC(cudaMallocHost(&d->h_results, sizeof(jb200_utt_result) * max_utts));
-  TRYC(cudaMallocHost(&d->h_atoms, sizeof(jb200_atom) * (size_t)d->atoms_cap));
-  TRYC(cudaMallocHost(&d->h_words, sizeof(int) * (size_t)max_utts * MAX_WORDS));
-  TRYC(cudaMallocHost(&d->h_counter, sizeof(unsigned long long)));
-  TRY(dev_alloc(d, (size_t)jb200_decoder::MAX_CHUNKS * max_utts, &d->d_chunk));
-  TRYC(cudaMallocHost(&d->h_chunk, sizeof(ChunkDesc) * (size_t)jb200_decoder::MAX_CHUNKS * max_utts));
-  TRY(dev_alloc(d, (size_t)max_utts, &d->d_state));
-  TRYC(cudaMemset(d->d_state, 0, sizeof(UttState) * (size_t)max_utts));
-  TRY(dev_alloc(d, (size_t)max_utts * MAX_WORDS, &d->d_interim_words));
-  TRY(dev_alloc(d, (size_t)jb200_decoder::MAX_CHUNKS * (2 * max_utts + 1), &d->d_seg));
-  TRYC(cudaMallocHost(&d->h_seg, sizeof(int) * (size_t)jb200_decoder::MAX_CHUNKS * (2 * max_utts + 1)));
-  TRYC(cudaMallocHost(&d->h_aoff, sizeof(long long) * (size_t)(max_utts + 1)));
-  TRYC(cudaMallocHost(&d->h_state, sizeof(UttState) * (size_t)max_utts));
-  TRYC(cudaMallocHost(&d->h_interim_words, sizeof(int) * (size_t)max_utts * MAX_WORDS));
-  {
-    // the scoring stream of the batch pipeline gets the higher priority: its thread blocks take the room the token-passing
-    // kernel leaves on every SM as soon as it is free
-    int lo = 0, hi = 0;
-    TRYC(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    TRYC(cudaStreamCreateWithPriority(&d->score_stream, cudaStreamNonBlocking, hi));
-    for (auto &e : d->ev_slice) TRYC(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    TRYC(cudaEventCreate(&d->ev_score_begin)); TRYC(cudaEventCreate(&d->ev_score_end));
-    d->pipe_frames = 0;
-    if (const char *e = getenv("JB200_PIPE_FRAMES")) d->pipe_frames = std::max(0, atoi(e));
-  }
-  d->smem_bytes = (heap_global ? (size_t)P.qcap * 8 + (size_t)(t->beam_width + 2) * 8 : (size_t)(maxt + 4) * 8) + offs_bytes;
-  d->beam = beam_kernel_for(grammar, P.multipath, check_heap);
+  JB_RC(reset_slots(d, 0, mu));
+  P.atoms_out_cap = (long long)mf * d->atoms_per_frame + (long long)mu * 64;
+  const size_t atoms_cap = (size_t)P.atoms_out_cap;
+  JB_RC(dev_alloc(d, atoms_cap, &P.atoms_raw));
+  JB_RC(dev_alloc(d, atoms_cap, &P.newidx));
+  JB_RC(dev_alloc(d, (size_t)mf + mu + 8, &P.group0));
+  JB_RC(dev_alloc(d, (size_t)mf * 2 + 8, &P.counts));
+  JB_RC(dev_alloc(d, atoms_cap, &P.atoms_out));
+  JB_RC(dev_alloc(d, 1, &P.atom_counter));
+  JB_RC(dev_alloc(d, (size_t)mu, &P.results));
+  JB_RC(dev_alloc(d, (size_t)mu * MAX_WORDS, &P.words));
+  JB_RC(dev_alloc(d, (size_t)mu * 8, &P.prof));
+  JB_RC(dev_alloc(d, (size_t)mu + 1, &d->d_frame_off));
+  JB_RC(dev_alloc(d, (size_t)mu + 1, &d->d_atom_off));
+  JB_RC(dev_alloc(d, (size_t)mf * d->dim, &d->d_feats));
+  JB_RC(dev_alloc(d, (size_t)mf * P.row_stride, &d->d_rows));
+  JB_RC(host_alloc(d, (size_t)mu, &d->h_results));
+  JB_RC(host_alloc(d, atoms_cap, &d->h_atoms));
+  JB_RC(host_alloc(d, (size_t)mu * MAX_WORDS, &d->h_words));
+  JB_RC(host_alloc(d, 1, &d->h_counter));
+  JB_RC(dev_alloc(d, (size_t)MC * mu, &d->d_chunk));
+  JB_RC(host_alloc(d, (size_t)MC * mu, &d->h_chunk));
+  JB_RC(dev_alloc(d, (size_t)mu, &P.state));
+  JB_CUDA(cudaMemset(P.state, 0, sizeof(UttState) * (size_t)mu));
+  JB_RC(dev_alloc(d, (size_t)mu * MAX_WORDS, &P.interim_words));
+  JB_RC(dev_alloc(d, (size_t)MC * (2 * mu + 1), &d->d_seg));
+  JB_RC(host_alloc(d, (size_t)MC * (2 * mu + 1), &d->h_seg));
+  JB_RC(host_alloc(d, (size_t)mu + 1, &d->h_aoff));
+  JB_RC(host_alloc(d, (size_t)mu, &d->h_state));
+  JB_RC(host_alloc(d, (size_t)mu * MAX_WORDS, &d->h_interim_words));
+  P.rows = d->d_rows; P.frame_off = d->d_frame_off; P.atom_off = d->d_atom_off; P.chunk = d->d_chunk;
+  // the scoring stream of the batch pipeline gets the higher priority: its thread blocks take the room the token-passing
+  // kernel leaves on every SM as soon as it is free
+  int lo = 0, hi = 0;
+  JB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+  JB_CUDA(cudaStreamCreateWithPriority(&d->score_stream, cudaStreamNonBlocking, hi));
+  for (auto &e : d->ev_slice) JB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  JB_CUDA(cudaEventCreate(&d->ev_score_begin)); JB_CUDA(cudaEventCreate(&d->ev_score_end));
+  if (const char *e = getenv("JB200_PIPE_FRAMES")) d->pipe_frames = std::max(0, atoi(e));
+  d->smem_bytes = cs.smem_bytes;
+  d->beam = beam_kernel_for(t->lm_type == JB200_LM_DFA, P.multipath, check_heap);
   const void *kern = (const void *)d->beam;
-  TRYC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
-  {
-    int per_sm = 0, sms = 0;
-    TRYC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BEAM_THREADS, d->smem_bytes));
-    TRYC(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d->device));
-    d->resident = per_sm * sms;
-  }
-  TRYC(cudaStreamSynchronize(d->stream));
-#undef TRY
-#undef TRYC
+  JB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
+  int per_sm = 0, sms = 0;
+  JB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BEAM_THREADS, d->smem_bytes));
+  JB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d->device));
+  d->resident = per_sm * sms;
+  JB_CUDA(cudaStreamSynchronize(d->stream));
+  return JB200_OK;
+}
+
+// the device half of jb200_decoder_create, on a checked tree
+static int build_decoder(jb200_decoder *d, const jb200_tree_desc *t, jb200_gmm *am, int max_utts, int max_frames) {
+  d->am = am; d->device = gmm_device(am); d->dim = gmm_dim(am); d->S = jb200_gmm_n_states(am);
+  d->P.row_stride = (d->S + 3) & ~3;
+  d->max_utts = max_utts; d->max_frames = max_frames;
+  if (const char *e = getenv("JB200_ATOMS_PER_FRAME")) d->atoms_per_frame = std::max(4, atoi(e));
+  JB_CUDA(cudaSetDevice(d->device));
+  JB_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
+  for (auto &e : d->ev) JB_CUDA(cudaEventCreate(&e));
+  // bigram-factoring memo, 2^21 entries: keys are (word id, successor slot) packed 16+16, so it needs both below 65535
+  d->P.lmc_bits = (t->n_words >= 65535 || t->n_scword >= 65535) ? 0 : 21;
+  // shared read-only tables: nodes 32 B, arcs 8 B, context table, inter-word table, bigram memo, LM arrays (+ slack)
+  const size_t est = (size_t)t->n_nodes * 32 + (size_t)t->n_arcs * 8 * 3 + (size_t)t->n_rset * (t->n_ctx + 1) * 4 + (size_t)t->n_words * 32 +
+                     (size_t)t->n_words * std::max(t->n_iso, 1) * (t->lm_type == JB200_LM_DFA ? 1 : 4) + ((size_t)8 << d->P.lmc_bits) +
+                     (size_t)t->lm_nvocab * 16 + (size_t)t->lm_nbigram * 8 + (size_t)(t->n_iso + t->n_shared + t->n_fscore + t->n_scword) * 16 + (4u << 20);
+  if (cudaMalloc(&d->arena, est) == cudaSuccess) { d->arena_size = est; d->dev_allocs.push_back(d->arena); }
+  else { d->arena = nullptr; cudaGetLastError(); }
+  JB_RC(upload_tree(d, t));
+  JB_RC(upload_lm(d, t));
+  int smem_optin = 0;
+  JB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->device));
+  CutSizing cs;
+  JB_RC(size_cut(t->beam_width, t->n_start, smem_optin, &cs));
+  return alloc_work(d, t, cs);
+}
+
+extern "C" int jb200_decoder_create(const jb200_tree_desc *t, jb200_gmm *am, int max_utts, int max_frames, jb200_decoder **out) {
+  if (!t || !out || max_utts < 1 || max_frames < 1) { set_error("jb200_decoder_create: bad argument"); return JB200_ERR_ARG; }
+  JB_RC(check_tree(t));
+  if (!am) { set_error("jb200_decoder_create: no acoustic model"); return JB200_ERR_ARG; }
+  jb200_decoder *d = new jb200_decoder();
+  const int rc = build_decoder(d, t, am, max_utts, max_frames);
+  if (rc) { jb200_decoder_destroy(d); return rc; }
   *out = d;
+  return JB200_OK;
+}
+
+// Lays out n_utts utterances: frame_off (n_utts + 1 entries) becomes h_frame_off, and an utterance of T frames gets room
+// for T * atoms_per_frame + 64 atoms from h_aoff[u] on.  Both go to the device on the main stream.
+static int layout_utts(jb200_decoder *d, const int32_t *frame_off, int n_utts) {
+  d->h_aoff[0] = 0;
+  for (int u = 0; u < n_utts; u++) {
+    const int T = frame_off[u + 1] - frame_off[u];
+    if (T < 0 || T > 32767) { set_error("utterance %d has %d frames (trellis times are 16-bit in the reference)", u, T); return JB200_ERR_ARG; }
+    d->h_aoff[u + 1] = d->h_aoff[u] + (long long)T * d->atoms_per_frame + 64;
+  }
+  d->h_frame_off.assign(frame_off, frame_off + n_utts + 1);
+  JB_CUDA(cudaMemcpyAsync(d->d_frame_off, d->h_frame_off.data(), sizeof(int) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
+  JB_CUDA(cudaMemcpyAsync(d->d_atom_off, d->h_aoff, sizeof(long long) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
   return JB200_OK;
 }
 
 // Cut a batch into time slices.  One slice (the whole utterance per launch) unless the pipeline is on: then slice c holds
 // frames [c*F, (c+1)*F) of every utterance, scored by its own launch on the scoring stream (a gather over the segment
 // list) while the beam kernel works on slice c-1.  Fills the staging copies of the chunk descriptors and segment lists.
-static int plan_slices(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
+static void plan_slices(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
   int maxT = 0;
   for (int u = 0; u < n_utts; u++) maxT = std::max(maxT, frame_off[u + 1] - frame_off[u]);
   int F = (allow_pipe && !d->dnn && d->pipe_frames > 0) ? d->pipe_frames : 0;
@@ -2466,10 +2525,9 @@ static int plan_slices(jb200_decoder *d, const int32_t *frame_off, int n_utts, b
     so[nseg] = lf;
     d->slice_nseg[c] = nseg; d->slice_frames[c] = lf;
   }
-  return JB200_OK;
 }
 
-static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe = true) {
+static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
   if (!d || !frame_off || n_utts < 1) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
   if (n_utts > d->max_utts) { set_error("batch of %d utterances exceeds decoder capacity %d", n_utts, d->max_utts); return JB200_ERR_CAPACITY; }
   const int total = frame_off[n_utts] - frame_off[0];
@@ -2477,89 +2535,81 @@ static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts,
   if (total > d->max_frames) { set_error("batch of %d frames exceeds decoder capacity %d", total, d->max_frames); return JB200_ERR_CAPACITY; }
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaStreamSynchronize(d->stream));   // the staging buffers below may still feed the previous batch's copies
-  d->h_aoff[0] = 0;
-  for (int u = 0; u < n_utts; u++) {
-    const int T = frame_off[u + 1] - frame_off[u];
-    if (T < 0 || T > 32767) { set_error("utterance %d has %d frames (trellis times are 16-bit in the reference)", u, T); return JB200_ERR_ARG; }
-    d->h_aoff[u + 1] = d->h_aoff[u] + (long long)T * d->atoms_per_frame + 64;
-  }
+  JB_RC(layout_utts(d, frame_off, n_utts));
   d->stream_mode = false;
-  d->h_frame_off.assign(frame_off, frame_off + n_utts + 1);
-  int rc = plan_slices(d, frame_off, n_utts, allow_pipe); if (rc) return rc;
+  plan_slices(d, frame_off, n_utts, allow_pipe);
   const int mu = d->max_utts;
-  JB_CUDA(cudaMemcpyAsync(d->d_frame_off, d->h_frame_off.data(), sizeof(int) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->d_atom_off, d->h_aoff, sizeof(long long) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
   JB_CUDA(cudaMemcpyAsync(d->d_chunk, d->h_chunk, sizeof(ChunkDesc) * (size_t)d->n_chunks * mu, cudaMemcpyHostToDevice, d->stream));
   if (d->last_piped)
     JB_CUDA(cudaMemcpyAsync(d->d_seg, d->h_seg, sizeof(int) * (size_t)d->n_chunks * (2 * mu + 1), cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaMemsetAsync(d->d_atom_counter, 0, sizeof(unsigned long long), d->stream));
+  JB_CUDA(cudaMemsetAsync(d->P.atom_counter, 0, sizeof(unsigned long long), d->stream));
   JB_CUDA(cudaStreamSynchronize(d->stream));   // h_frame_off is a std::vector (pageable)
   d->last_n = n_utts; d->last_total_frames = total; d->fetched = false;
   return JB200_OK;
 }
 
-static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index = 0, int interim = 0) {
+static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index, int interim = 0) {
   BeamParams P = d->P;
-  P.rows = d->d_rows; P.row_stride = d->row_stride; P.frame_off = d->d_frame_off;
-  P.atom_off = d->d_atom_off; P.atoms_out = d->d_atoms_out; P.atom_counter = d->d_atom_counter;
-  P.atoms_out_cap = d->atoms_cap; P.results = d->d_results; P.words = d->d_words; P.prof = d->d_prof;
-  P.chunk = d->d_chunk + (size_t)chunk_index * d->max_utts; P.state = d->d_state;
-  P.interim = interim; P.interim_words = d->d_interim_words; P.atoms_in_place = d->stream_mode ? 1 : 0;
+  P.chunk = d->d_chunk + (size_t)chunk_index * d->max_utts;
+  P.interim = interim; P.atoms_in_place = d->stream_mode ? 1 : 0;
   d->beam<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
   JB_LAUNCH_CHECK();
   return JB200_OK;
 }
 
-// scoring + token passing of a prepared batch whose features are at d_feats; ev[1] has been recorded on the main stream
-static int run_batch(jb200_decoder *d, const float *d_feats, int n_utts) {
-  int rc;
-  if (!d->last_piped) {
-    rc = d->dnn ? dnn_forward_device(d->dnn, d_feats, d->last_total_frames, d->d_rows, d->row_stride, d->stream)
-                : gmm_launch_states(d->am, d_feats, d->last_total_frames, d->d_rows, d->row_stride, d->stream, nullptr, nullptr, 0);
-    if (rc) return rc;
-    JB_CUDA(cudaEventRecord(d->ev[2], d->stream));
-    return launch_beam(d, n_utts, 0);
-  }
-  // pipeline: every slice's scoring is queued on the scoring stream at once (it only depends on the features), the beam
-  // kernel of slice c waits for the scores of slice c alone
+// scores T frames of device features into the score rows, on the main stream
+static int score_frames(jb200_decoder *d, const float *d_feats, int T) {
+  return d->dnn ? dnn_forward_device(d->dnn, d_feats, T, d->d_rows, d->P.row_stride, d->stream)
+                : gmm_launch_states(d->am, d_feats, T, d->d_rows, d->P.row_stride, d->stream, nullptr, nullptr, 0);
+}
+
+// scoring of a prepared batch's features at d_feats, time slice by time slice on the scoring stream, beside the token
+// passing of the slices on the main stream; ev[1] has been recorded on the main stream
+static int run_pipeline(jb200_decoder *d, const float *d_feats, int n_utts) {
+  // every slice's scoring is queued on the scoring stream at once (it only depends on the features), the beam kernel of
+  // slice c waits for the scores of slice c alone
   const int mu = d->max_utts, segw = 2 * mu + 1;
   JB_CUDA(cudaStreamWaitEvent(d->score_stream, d->ev[1], 0));
   JB_CUDA(cudaEventRecord(d->ev_score_begin, d->score_stream));
   for (int c = 0; c < d->n_chunks; c++) {
     const int *ds = d->d_seg + (size_t)c * segw;
-    rc = gmm_launch_states(d->am, d_feats, d->slice_frames[c], d->d_rows, d->row_stride, d->score_stream, ds, ds + mu + 1, d->slice_nseg[c]);
-    if (rc) return rc;
+    JB_RC(gmm_launch_states(d->am, d_feats, d->slice_frames[c], d->d_rows, d->P.row_stride, d->score_stream, ds, ds + mu + 1, d->slice_nseg[c]));
     JB_CUDA(cudaEventRecord(d->ev_slice[c], d->score_stream));
   }
   JB_CUDA(cudaEventRecord(d->ev_score_end, d->score_stream));
   for (int c = 0; c < d->n_chunks; c++) {
     JB_CUDA(cudaStreamWaitEvent(d->stream, d->ev_slice[c], 0));
     if (c == 0) JB_CUDA(cudaEventRecord(d->ev[2], d->stream));       // "scoring" = what the beam had to wait for
-    rc = launch_beam(d, n_utts, c); if (rc) return rc;
+    JB_RC(launch_beam(d, n_utts, c));
   }
   return JB200_OK;
+}
+
+// The phase times of the last batch: ev[0..4] bracket the upload, the scoring, the beam and the copy of the results.
+// The last is 0 when the results were not fetched.
+static void read_timing(jb200_decoder *d, bool fetched) {
+  for (int i = 0; i < 3; i++) cudaEventElapsedTime(&d->last_ms[i], d->ev[i], d->ev[i + 1]);
+  d->last_ms[3] = 0.0f;
+  if (fetched) cudaEventElapsedTime(&d->last_ms[3], d->ev[3], d->ev[4]);
+  if (d->last_piped) cudaEventElapsedTime(&d->last_score_busy_ms, d->ev_score_begin, d->ev_score_end);
 }
 
 extern "C" int jb200_decoder_fetch(jb200_decoder *d) {
   if (!d) { set_error("null decoder"); return JB200_ERR_ARG; }
   if (d->fetched) return JB200_OK;
+  const BeamParams &P = d->P;
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaEventRecord(d->ev[3], d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->h_counter, d->d_atom_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->h_results, d->d_results, sizeof(jb200_utt_result) * d->last_n, cudaMemcpyDeviceToHost, d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->h_words, d->d_words, sizeof(int) * (size_t)d->last_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
+  JB_CUDA(cudaMemcpyAsync(d->h_counter, P.atom_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, d->stream));
+  JB_CUDA(cudaMemcpyAsync(d->h_results, P.results, sizeof(jb200_utt_result) * d->last_n, cudaMemcpyDeviceToHost, d->stream));
+  JB_CUDA(cudaMemcpyAsync(d->h_words, P.words, sizeof(int) * (size_t)d->last_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
   JB_CUDA(cudaStreamSynchronize(d->stream));
   long long na = (long long)*d->h_counter;
-  if (na > d->atoms_cap) na = d->atoms_cap;
-  d->last_atoms = na;
-  if (na > 0) JB_CUDA(cudaMemcpyAsync(d->h_atoms, d->d_atoms_out, sizeof(jb200_atom) * (size_t)na, cudaMemcpyDeviceToHost, d->stream));
+  if (na > P.atoms_out_cap) na = P.atoms_out_cap;
+  if (na > 0) JB_CUDA(cudaMemcpyAsync(d->h_atoms, P.atoms_out, sizeof(jb200_atom) * (size_t)na, cudaMemcpyDeviceToHost, d->stream));
   JB_CUDA(cudaEventRecord(d->ev[4], d->stream));
   JB_CUDA(cudaStreamSynchronize(d->stream));
-  cudaEventElapsedTime(&d->last_ms[0], d->ev[0], d->ev[1]);
-  cudaEventElapsedTime(&d->last_ms[1], d->ev[1], d->ev[2]);
-  cudaEventElapsedTime(&d->last_ms[2], d->ev[2], d->ev[3]);
-  cudaEventElapsedTime(&d->last_ms[3], d->ev[3], d->ev[4]);
-  if (d->last_piped) cudaEventElapsedTime(&d->last_score_busy_ms, d->ev_score_begin, d->ev_score_end);
+  read_timing(d, true);
   d->last_d2h = (long long)sizeof(unsigned long long) + (long long)sizeof(jb200_utt_result) * d->last_n +
                 (long long)sizeof(int) * d->last_n * MAX_WORDS + (long long)sizeof(jb200_atom) * na;
   d->fetched = true;
@@ -2570,23 +2620,17 @@ extern "C" int jb200_decoder_sync_timing(jb200_decoder *d) {
   if (!d) { set_error("null decoder"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaEventSynchronize(d->ev[3]));
-  cudaEventElapsedTime(&d->last_ms[0], d->ev[0], d->ev[1]);
-  cudaEventElapsedTime(&d->last_ms[1], d->ev[1], d->ev[2]);
-  cudaEventElapsedTime(&d->last_ms[2], d->ev[2], d->ev[3]);
-  if (d->last_piped) cudaEventElapsedTime(&d->last_score_busy_ms, d->ev_score_begin, d->ev_score_end);
-  d->last_ms[3] = 0.0f;
+  read_timing(d, false);
   return JB200_OK;
 }
 
 extern "C" int jb200_decoder_phase_cycles(jb200_decoder *d, int64_t *cycles, int n_utts) {
   if (!d || !cycles || n_utts < 1 || n_utts > d->last_n) { set_error("bad argument"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
-  JB_CUDA(cudaMemcpy(cycles, d->d_prof, sizeof(long long) * 8 * (size_t)n_utts, cudaMemcpyDeviceToHost));
+  JB_CUDA(cudaMemcpy(cycles, d->P.prof, sizeof(long long) * 8 * (size_t)n_utts, cudaMemcpyDeviceToHost));
   return JB200_OK;
 }
 
-extern "C" int jb200_dnn_in_dim(const jb200_dnn *h);
-extern "C" int jb200_dnn_out_dim(const jb200_dnn *h);
 extern "C" int jb200_decoder_attach_dnn(jb200_decoder *d, jb200_dnn *dnn) {
   if (!d || !dnn) { set_error("null argument"); return JB200_ERR_ARG; }
   if (jb200_dnn_out_dim(dnn) != d->S) { set_error("DNN has %d outputs but the HMM set has %d states", jb200_dnn_out_dim(dnn), d->S); return JB200_ERR_ARG; }
@@ -2595,89 +2639,90 @@ extern "C" int jb200_decoder_attach_dnn(jb200_decoder *d, jb200_dnn *dnn) {
   if (dim != d->dim) {
     // the feature buffer was sized for the AM's dimension; re-size it for the DNN's input width
     float *nf = nullptr;
-    JB_CUDA(cudaMalloc(&nf, sizeof(float) * (size_t)d->max_frames * dim));
-    d->dev_allocs.push_back(nf);
+    JB_RC(dev_alloc(d, (size_t)d->max_frames * dim, &nf));
     d->d_feats = nf; d->dim = dim;
   }
   d->dnn = dnn;
   return JB200_OK;
 }
 
+// copies the beam-cut counters [first, first + n) to out
+static int read_cut_counters(jb200_decoder *d, CutCounter first, int n, int64_t *out) {
+  if (!d || !out) { set_error("bad argument"); return JB200_ERR_ARG; }
+  unsigned long long v[CUT_SLOTS];
+  JB_CUDA(cudaSetDevice(d->device));
+  JB_CUDA(cudaMemcpy(v, d->P.cut_counters + first, sizeof(v[0]) * n, cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n; i++) out[i] = (int64_t)v[i];
+  return JB200_OK;
+}
+
 extern "C" int64_t jb200_decoder_misspeculations(jb200_decoder *d) {
-  if (!d) return -1;
-  unsigned long long v = 0;
-  cudaSetDevice(d->device);
-  if (cudaMemcpy(&v, d->P.misspec_counter, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-  return (int64_t)v;
+  int64_t v = 0;
+  return read_cut_counters(d, CUT_SEQ_FALLBACKS, 1, &v) == JB200_OK ? v : -1;
 }
 
 extern "C" int jb200_decoder_heap_stats(jb200_decoder *d, int64_t out[3]) {
-  if (!d || !out) { set_error("bad argument"); return JB200_ERR_ARG; }
-  unsigned long long v[3] = {0, 0, 0};
-  JB_CUDA(cudaSetDevice(d->device));
-  JB_CUDA(cudaMemcpy(v, d->P.misspec_counter, sizeof(v), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < 3; i++) out[i] = (int64_t)v[i];
-  return JB200_OK;
+  return read_cut_counters(d, CUT_SEQ_FALLBACKS, 3, out);     // fall-backs, replay ticks, extractions replayed
 }
 
 extern "C" int jb200_decoder_select_stats(jb200_decoder *d, int64_t out[2]) {
-  if (!d || !out) { set_error("bad argument"); return JB200_ERR_ARG; }
-  unsigned long long v[2] = {0, 0};
-  JB_CUDA(cudaSetDevice(d->device));
-  JB_CUDA(cudaMemcpy(v, d->P.misspec_counter + 4, sizeof(v), cudaMemcpyDeviceToHost));
-  out[0] = (int64_t)v[0]; out[1] = (int64_t)v[1];
-  return JB200_OK;
+  return read_cut_counters(d, CUT_UPWARD, 2, out);            // upward selects, of which closed form
 }
 
 extern "C" int64_t jb200_decoder_relocated_selects(jb200_decoder *d) {
-  if (!d) return -1;
-  unsigned long long v = 0;
-  cudaSetDevice(d->device);
-  if (cudaMemcpy(&v, d->P.misspec_counter + 6, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-  return (int64_t)v;
+  int64_t v = 0;
+  return read_cut_counters(d, CUT_RELOCATED, 1, &v) == JB200_OK ? v : -1;
 }
 
 extern "C" int jb200_decoder_cut_placement(jb200_decoder *d, int64_t out[3]) {
   if (!d || !out) { set_error("bad argument"); return JB200_ERR_ARG; }
-  unsigned long long v[2] = {0, 0};
-  JB_CUDA(cudaSetDevice(d->device));
-  JB_CUDA(cudaMemcpy(v, d->P.misspec_counter + 7, sizeof(v), cudaMemcpyDeviceToHost));
-  out[0] = d->P.heap_g ? 1 : 0; out[1] = (int64_t)v[0]; out[2] = (int64_t)v[1];
+  JB_RC(read_cut_counters(d, CUT_GLOBAL_WHOLE, 2, out + 1));  // whole-heap copies, top-and-tail copies
+  out[0] = d->P.heap_g ? 1 : 0;
   return JB200_OK;
 }
 
 extern "C" int64_t jb200_decoder_last_d2h_bytes(const jb200_decoder *d) { return d ? d->last_d2h : 0; }
 extern "C" int jb200_decoder_resident_utts(const jb200_decoder *d) { return d ? d->resident : 0; }
 
-extern "C" int jb200_decode_batch_device(jb200_decoder *d, const float *d_feats, const int32_t *frame_off, int n_utts) {
-  int rc = prepare_batch(d, frame_off, n_utts); if (rc) return rc;
+// What a batch call hands in: features on the device, features on the host, or score rows on the host
+enum BatchInput { FEATS_DEVICE, FEATS_HOST, SCORES_HOST };
+
+// One batch, ev[0..3] around the upload, the scoring and the beam.  The host variants fetch the results; for device
+// features that is left to jb200_decoder_fetch.  Score rows are never pipelined.
+static int decode_batch(jb200_decoder *d, BatchInput in, const float *x, const int32_t *frame_off, int n_utts) {
+  if (in != FEATS_DEVICE && !x) { set_error(in == SCORES_HOST ? "null scores" : "null feats"); return JB200_ERR_ARG; }
+  JB_RC(prepare_batch(d, frame_off, n_utts, in != SCORES_HOST));
   JB_CUDA(cudaEventRecord(d->ev[0], d->stream));
+  if (in == FEATS_HOST) {
+    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)d->last_total_frames * d->dim, cudaMemcpyHostToDevice, d->stream));
+    x = d->d_feats;
+  }
+  if (in == SCORES_HOST)
+    JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->P.row_stride, x, sizeof(float) * d->S, sizeof(float) * d->S,
+                              d->last_total_frames, cudaMemcpyHostToDevice, d->stream));
   JB_CUDA(cudaEventRecord(d->ev[1], d->stream));
-  rc = run_batch(d, d_feats, n_utts); if (rc) return rc;
+  if (d->last_piped) {
+    JB_RC(run_pipeline(d, x, n_utts));
+  } else {
+    if (in != SCORES_HOST) JB_RC(score_frames(d, x, d->last_total_frames));
+    JB_CUDA(cudaEventRecord(d->ev[2], d->stream));
+    JB_RC(launch_beam(d, n_utts, 0));
+  }
+  if (in != FEATS_DEVICE) return jb200_decoder_fetch(d);
   JB_CUDA(cudaEventRecord(d->ev[3], d->stream));
   return JB200_OK;
 }
 
+extern "C" int jb200_decode_batch_device(jb200_decoder *d, const float *d_feats, const int32_t *frame_off, int n_utts) {
+  return decode_batch(d, FEATS_DEVICE, d_feats, frame_off, n_utts);
+}
+
 extern "C" int jb200_decode_batch_host(jb200_decoder *d, const float *feats, const int32_t *frame_off, int n_utts) {
-  if (!feats) { set_error("null feats"); return JB200_ERR_ARG; }
-  int rc = prepare_batch(d, frame_off, n_utts); if (rc) return rc;
-  JB_CUDA(cudaEventRecord(d->ev[0], d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->d_feats, feats, sizeof(float) * (size_t)d->last_total_frames * d->dim, cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaEventRecord(d->ev[1], d->stream));
-  rc = run_batch(d, d->d_feats, n_utts); if (rc) return rc;
-  return jb200_decoder_fetch(d);
+  return decode_batch(d, FEATS_HOST, feats, frame_off, n_utts);
 }
 
 extern "C" int jb200_decode_batch_scores_host(jb200_decoder *d, const float *scores, const int32_t *frame_off, int n_utts) {
-  if (!scores) { set_error("null scores"); return JB200_ERR_ARG; }
-  int rc = prepare_batch(d, frame_off, n_utts, false); if (rc) return rc;
-  JB_CUDA(cudaEventRecord(d->ev[0], d->stream));
-  JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->row_stride, scores, sizeof(float) * d->S, sizeof(float) * d->S,
-                            d->last_total_frames, cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaEventRecord(d->ev[1], d->stream));
-  JB_CUDA(cudaEventRecord(d->ev[2], d->stream));
-  rc = launch_beam(d, n_utts, 0); if (rc) return rc;
-  return jb200_decoder_fetch(d);
+  return decode_batch(d, SCORES_HOST, scores, frame_off, n_utts);
 }
 
 // ---- frame-synchronous operation (streams) -----------------------------------------------------------------------
@@ -2687,33 +2732,24 @@ extern "C" int jb200_stream_open(jb200_decoder *d, int n_streams) {
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaStreamSynchronize(d->stream));
   // a stream that was abandoned before its last frame has left node slots behind: wipe those work areas
-  if (d->stream_mode) {
-    for (int u = 0; u < d->st_n; u++) if (d->st_started[u] && !d->st_done[u]) {
-      const size_t tot = (size_t)d->P.n_nodes;
-      fill_slots_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(d->P.slots + (size_t)u * d->P.n_nodes, tot);
-      JB_LAUNCH_CHECK();
-    }
-  }
+  if (d->stream_mode)
+    for (int u = 0; u < d->st_n; u++) if (d->st_started[u] && !d->st_done[u]) JB_RC(reset_slots(d, u, 1));
   const int cap = std::min(d->max_frames / n_streams, 32767);
   if (cap < 1) { set_error("decoder capacity of %d frames is too small for %d streams", d->max_frames, n_streams); return JB200_ERR_CAPACITY; }
   d->stream_mode = true; d->st_n = n_streams; d->st_cap = cap;
   d->st_t.assign(n_streams, 0); d->st_started.assign(n_streams, 0); d->st_done.assign(n_streams, 0);
-  d->h_frame_off.assign(n_streams + 1, 0);
-  d->h_aoff[0] = 0;
-  for (int u = 0; u < n_streams; u++) {
-    d->h_frame_off[u + 1] = d->h_frame_off[u] + cap;
-    d->h_aoff[u + 1] = d->h_aoff[u] + (long long)cap * d->atoms_per_frame + 64;
-  }
-  JB_CUDA(cudaMemcpyAsync(d->d_frame_off, d->h_frame_off.data(), sizeof(int) * (n_streams + 1), cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaMemcpyAsync(d->d_atom_off, d->h_aoff, sizeof(long long) * (n_streams + 1), cudaMemcpyHostToDevice, d->stream));
+  std::vector<int32_t> frame_off(n_streams + 1);
+  for (int u = 0; u <= n_streams; u++) frame_off[u] = u * cap;
+  JB_RC(layout_utts(d, frame_off.data(), n_streams));
   JB_CUDA(cudaStreamSynchronize(d->stream));
   d->last_n = n_streams; d->n_chunks = 1; d->last_piped = false; d->fetched = true;
   return JB200_OK;
 }
 
-// device part shared by the feature / score variants: rows of the new frames are in d_rows, packed stream-major
+// device part of a feed: rows of the new frames are in d_rows, packed stream-major
 static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t *last, int want_interim) {
-  int pack = 0, any = 0;
+  int pack = 0;
+  bool any = false, fin_any = false;
   for (int u = 0; u < d->st_n; u++) {
     ChunkDesc k; k.t0 = d->st_t[u]; k.t1 = k.t0 + n_new[u]; k.row_base = pack - k.t0; k.flags = 0;
     const bool fin = last && last[u];
@@ -2721,24 +2757,23 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
     else {
       if (!d->st_started[u]) k.flags |= CHUNK_FIRST;
       if (fin) k.flags |= CHUNK_FINAL;
-      any = 1;
+      any = true; fin_any |= fin;
     }
     d->h_chunk[u] = k;
     pack += n_new[u];
   }
   if (!any) return JB200_OK;
+  const BeamParams &P = d->P;
   JB_CUDA(cudaMemcpyAsync(d->d_chunk, d->h_chunk, sizeof(ChunkDesc) * (size_t)d->st_n, cudaMemcpyHostToDevice, d->stream));
-  int rc = launch_beam(d, d->st_n, 0, want_interim); if (rc) return rc;
+  JB_RC(launch_beam(d, d->st_n, 0, want_interim));
   // results of the streams that ended; interim state of the others
-  bool fin_any = false;
-  for (int u = 0; u < d->st_n; u++) if (d->h_chunk[u].flags & CHUNK_FINAL) fin_any = true;
   if (fin_any) {
-    JB_CUDA(cudaMemcpyAsync(d->h_results, d->d_results, sizeof(jb200_utt_result) * d->st_n, cudaMemcpyDeviceToHost, d->stream));
-    JB_CUDA(cudaMemcpyAsync(d->h_words, d->d_words, sizeof(int) * (size_t)d->st_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
+    JB_CUDA(cudaMemcpyAsync(d->h_results, P.results, sizeof(jb200_utt_result) * d->st_n, cudaMemcpyDeviceToHost, d->stream));
+    JB_CUDA(cudaMemcpyAsync(d->h_words, P.words, sizeof(int) * (size_t)d->st_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
   }
-  JB_CUDA(cudaMemcpyAsync(d->h_state, d->d_state, sizeof(UttState) * (size_t)d->st_n, cudaMemcpyDeviceToHost, d->stream));
+  JB_CUDA(cudaMemcpyAsync(d->h_state, P.state, sizeof(UttState) * (size_t)d->st_n, cudaMemcpyDeviceToHost, d->stream));
   if (want_interim)
-    JB_CUDA(cudaMemcpyAsync(d->h_interim_words, d->d_interim_words, sizeof(int) * (size_t)d->st_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
+    JB_CUDA(cudaMemcpyAsync(d->h_interim_words, P.interim_words, sizeof(int) * (size_t)d->st_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
   JB_CUDA(cudaStreamSynchronize(d->stream));
   d->last_d2h = 0;
   for (int u = 0; u < d->st_n; u++) {
@@ -2748,7 +2783,7 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
     if (fl & CHUNK_FINAL) {
       d->st_done[u] = 1;
       const int na = d->h_results[u].n_atoms;
-      if (na > 0) JB_CUDA(cudaMemcpyAsync(d->h_atoms + d->h_aoff[u], d->d_atoms_out + d->h_aoff[u], sizeof(jb200_atom) * (size_t)na, cudaMemcpyDeviceToHost, d->stream));
+      if (na > 0) JB_CUDA(cudaMemcpyAsync(d->h_atoms + d->h_aoff[u], P.atoms_out + d->h_aoff[u], sizeof(jb200_atom) * (size_t)na, cudaMemcpyDeviceToHost, d->stream));
       d->last_d2h += (long long)sizeof(jb200_atom) * na + (long long)sizeof(jb200_utt_result) + (long long)sizeof(int) * MAX_WORDS;
     }
   }
@@ -2756,7 +2791,8 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
   return JB200_OK;
 }
 
-static int stream_check(jb200_decoder *d, const int32_t *n_new, int *total) {
+// jb200_stream_feed_host / _scores_host: the new frames of every stream, packed stream-major, as features or as score rows
+static int stream_feed(jb200_decoder *d, bool scores, const float *x, const int32_t *n_new, const uint8_t *last, int want_interim) {
   if (!d || !n_new) { set_error("jb200_stream_feed: bad argument"); return JB200_ERR_ARG; }
   if (!d->stream_mode) { set_error("jb200_stream_feed: call jb200_stream_open first"); return JB200_ERR_ARG; }
   int tot = 0;
@@ -2767,41 +2803,30 @@ static int stream_check(jb200_decoder *d, const int32_t *n_new, int *total) {
     tot += n_new[u];
   }
   if (tot > d->max_frames) { set_error("%d new frames exceed decoder capacity %d", tot, d->max_frames); return JB200_ERR_CAPACITY; }
-  *total = tot;
-  return JB200_OK;
-}
-
-extern "C" int jb200_stream_feed_host(jb200_decoder *d, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim) {
-  int tot = 0;
-  int rc = stream_check(d, n_new, &tot); if (rc) return rc;
-  if (tot > 0 && !feats) { set_error("null feats"); return JB200_ERR_ARG; }
+  if (tot > 0 && !x) { set_error(scores ? "null scores" : "null feats"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
-  if (tot > 0) {
-    JB_CUDA(cudaMemcpyAsync(d->d_feats, feats, sizeof(float) * (size_t)tot * d->dim, cudaMemcpyHostToDevice, d->stream));
-    rc = d->dnn ? dnn_forward_device(d->dnn, d->d_feats, tot, d->d_rows, d->row_stride, d->stream)
-                : gmm_launch_states(d->am, d->d_feats, tot, d->d_rows, d->row_stride, d->stream, nullptr, nullptr, 0);
-    if (rc) return rc;
+  if (tot > 0 && scores)
+    JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->P.row_stride, x, sizeof(float) * d->S, sizeof(float) * d->S, tot, cudaMemcpyHostToDevice, d->stream));
+  else if (tot > 0) {
+    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)tot * d->dim, cudaMemcpyHostToDevice, d->stream));
+    JB_RC(score_frames(d, d->d_feats, tot));
   }
   return stream_advance(d, n_new, last, want_interim);
 }
 
+extern "C" int jb200_stream_feed_host(jb200_decoder *d, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim) {
+  return stream_feed(d, false, feats, n_new, last, want_interim);
+}
+
 extern "C" int jb200_stream_feed_scores_host(jb200_decoder *d, const float *scores, const int32_t *n_new, const uint8_t *last, int want_interim) {
-  int tot = 0;
-  int rc = stream_check(d, n_new, &tot); if (rc) return rc;
-  if (tot > 0 && !scores) { set_error("null scores"); return JB200_ERR_ARG; }
-  JB_CUDA(cudaSetDevice(d->device));
-  if (tot > 0)
-    JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->row_stride, scores, sizeof(float) * d->S, sizeof(float) * d->S, tot, cudaMemcpyHostToDevice, d->stream));
-  return stream_advance(d, n_new, last, want_interim);
+  return stream_feed(d, true, scores, n_new, last, want_interim);
 }
 
 extern "C" int jb200_stream_restart(jb200_decoder *d, int stream) {
   if (!d || !d->stream_mode || stream < 0 || stream >= d->st_n) { set_error("jb200_stream_restart: bad argument"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
   if (d->st_started[stream] && !d->st_done[stream]) {
-    const size_t tot = (size_t)d->P.n_nodes;
-    fill_slots_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, d->stream>>>(d->P.slots + (size_t)stream * d->P.n_nodes, tot);
-    JB_LAUNCH_CHECK();
+    JB_RC(reset_slots(d, stream, 1));
     JB_CUDA(cudaStreamSynchronize(d->stream));
   }
   d->st_t[stream] = 0; d->st_started[stream] = 0; d->st_done[stream] = 0;

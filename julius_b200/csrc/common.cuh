@@ -37,6 +37,13 @@ __device__ __forceinline__ float addlog_step_exact(float y, float x, const float
     }                                                                              \
   } while (0)
 
+// passes on a failed JB200_* return code
+#define JB_RC(expr)                                                                \
+  do {                                                                             \
+    const int _rc = (expr);                                                        \
+    if (_rc != JB200_OK) return _rc;                                               \
+  } while (0)
+
 #define JB_LAUNCH_CHECK()                                                          \
   do {                                                                             \
     jb200::g_launches.fetch_add(1, std::memory_order_relaxed);                     \

@@ -292,30 +292,12 @@ extern "C" void jb200_dnn_destroy(jb200_dnn *h) {
   delete h;
 }
 
-extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn **out) {
-  if (!d || !out || d->n_layers < 1 || d->n_layers > JB200_DNN_MAX_LAYERS) { set_error("jb200_dnn_create: bad argument"); return JB200_ERR_ARG; }
-  // the kernels trust these: the input copy is in_dim wide, the last layer writes layer_out[n-1] columns into rows
-  // padded from out_dim, and the prior and the score rows are out_dim wide
-  for (int l = 0; l < d->n_layers; l++)
-    if (d->layer_in[l] < 1 || d->layer_out[l] < 1) { set_error("jb200_dnn_create: layer %d is %d -> %d", l, d->layer_in[l], d->layer_out[l]); return JB200_ERR_ARG; }
-  if (d->in_dim != d->layer_in[0] || d->out_dim != d->layer_out[d->n_layers - 1]) {
-    set_error("jb200_dnn_create: net is %d -> %d but its layers take %d and give %d", d->in_dim, d->out_dim, d->layer_in[0], d->layer_out[d->n_layers - 1]);
-    return JB200_ERR_ARG;
-  }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (libjb200 has no CPU fallback)"); return JB200_ERR_NODEVICE; }
-  if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return JB200_ERR_ARG; }
-  JB_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  JB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) { set_error("device is sm_%d%d; the wgmma GEMM needs sm_90a", prop.major, prop.minor); return JB200_ERR_NODEVICE; }
-  jb200_dnn *h = new jb200_dnn();
-  h->device = device; h->n_layers = d->n_layers; h->in_dim = d->in_dim; h->out_dim = d->out_dim;
-  h->row_stride = (d->out_dim + 3) & ~3;
+// the device half of jb200_dnn_create
+static int dnn_build(jb200_dnn *h, const jb200_dnn_desc *d) {
   {
     void *fn = nullptr; cudaDriverEntryPointQueryResult qres;
     cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) { set_error("cuTensorMapEncodeTiled not available"); delete h; return JB200_ERR_CUDA; }
+    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) { set_error("cuTensorMapEncodeTiled not available"); return JB200_ERR_CUDA; }
     h->encode = (PFN_encodeTiled)fn;
   }
   JB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -324,7 +306,6 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
   for (int l = 0; l < d->n_layers; l++) {
     DnnLayerDev &L = h->L[l];
     L.in = d->layer_in[l]; L.out = d->layer_out[l]; L.ld_in = (L.in + 7) & ~7;
-    if (l > 0 && L.in != d->layer_out[l - 1]) { set_error("layer %d input %d != previous output %d", l, L.in, d->layer_out[l - 1]); jb200_dnn_destroy(h); return JB200_ERR_ARG; }
     if (l + 1 < d->n_layers) h->max_width = std::max(h->max_width, (L.out + 7) & ~7);
     std::vector<__nv_bfloat16> hi((size_t)L.out * L.ld_in), lo((size_t)L.out * L.ld_in);
     for (int r = 0; r < L.out; r++)
@@ -339,8 +320,8 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
     JB_CUDA(cudaMemcpy(L.w_lo, lo.data(), lo.size() * 2, cudaMemcpyHostToDevice));
     JB_CUDA(cudaMalloc(&L.bias, sizeof(float) * L.out));
     JB_CUDA(cudaMemcpy(L.bias, d->b[l], sizeof(float) * L.out, cudaMemcpyHostToDevice));
-    int rc = make_map(h, &L.map_w_hi, L.w_hi, L.out, L.ld_in, L.ld_in); if (rc) { jb200_dnn_destroy(h); return rc; }
-    rc = make_map(h, &L.map_w_lo, L.w_lo, L.out, L.ld_in, L.ld_in); if (rc) { jb200_dnn_destroy(h); return rc; }
+    JB_RC(make_map(h, &L.map_w_hi, L.w_hi, L.out, L.ld_in, L.ld_in));
+    JB_RC(make_map(h, &L.map_w_lo, L.w_lo, L.out, L.ld_in, L.ld_in));
   }
   JB_CUDA(cudaMalloc(&h->d_prior, sizeof(float) * d->out_dim));
   JB_CUDA(cudaMemcpy(h->d_prior, d->state_prior, sizeof(float) * d->out_dim, cudaMemcpyHostToDevice));
@@ -356,7 +337,34 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
   }
   h->ld_logits = (d->out_dim + 3) & ~3;
   JB_CUDA(cudaFuncSetAttribute(dnn_gemm_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  return JB200_OK;
+}
+
+extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn **out) {
+  if (!d || !out || d->n_layers < 1 || d->n_layers > JB200_DNN_MAX_LAYERS) { set_error("jb200_dnn_create: bad argument"); return JB200_ERR_ARG; }
+  // the kernels trust these: the input copy is in_dim wide, each layer reads what the one before wrote, the last layer
+  // writes layer_out[n-1] columns into rows padded from out_dim, and the prior and the score rows are out_dim wide
+  for (int l = 0; l < d->n_layers; l++) {
+    if (d->layer_in[l] < 1 || d->layer_out[l] < 1) { set_error("jb200_dnn_create: layer %d is %d -> %d", l, d->layer_in[l], d->layer_out[l]); return JB200_ERR_ARG; }
+    if (l > 0 && d->layer_in[l] != d->layer_out[l - 1]) { set_error("jb200_dnn_create: layer %d input %d != previous output %d", l, d->layer_in[l], d->layer_out[l - 1]); return JB200_ERR_ARG; }
+  }
+  if (d->in_dim != d->layer_in[0] || d->out_dim != d->layer_out[d->n_layers - 1]) {
+    set_error("jb200_dnn_create: net is %d -> %d but its layers take %d and give %d", d->in_dim, d->out_dim, d->layer_in[0], d->layer_out[d->n_layers - 1]);
+    return JB200_ERR_ARG;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (libjb200 has no CPU fallback)"); return JB200_ERR_NODEVICE; }
+  if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return JB200_ERR_ARG; }
+  JB_CUDA(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  JB_CUDA(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) { set_error("device is sm_%d%d; the wgmma GEMM needs sm_90a", prop.major, prop.minor); return JB200_ERR_NODEVICE; }
+  jb200_dnn *h = new jb200_dnn();
+  h->device = device; h->n_layers = d->n_layers; h->in_dim = d->in_dim; h->out_dim = d->out_dim;
+  h->row_stride = (d->out_dim + 3) & ~3;
   h->n_sm = prop.multiProcessorCount;
+  const int rc = dnn_build(h, d);
+  if (rc) { jb200_dnn_destroy(h); return rc; }
   *out = h;
   return JB200_OK;
 }

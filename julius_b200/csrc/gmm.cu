@@ -343,27 +343,17 @@ int gmm_cd_device(const jb200_gmm *h, const int **cd_off, const int **cd_states,
 }
 }
 
-extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, jb200_gmm **out) {
-  if (!d || !out) { set_error("jb200_gmm_create: null argument"); return JB200_ERR_ARG; }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (libjb200 has no CPU fallback)"); return JB200_ERR_NODEVICE; }
-  if (device < 0 || device >= ndev) { set_error("device %d out of range (%d devices)", device, ndev); return JB200_ERR_ARG; }
-  if (d->gprune_method != JB200_GPRUNE_NONE && (d->gprune_num < 1 || d->gprune_num > GMM_NMAX)) {
-    set_error("-tmix %d outside supported range 1..%d", d->gprune_num, GMM_NMAX); return JB200_ERR_UNSUPPORTED;
-  }
-  if (d->iwcd_method == JB200_IWCD_NBEST && d->iwcd_nbest > GMM_NMAX) { set_error("-iwcd1 best %d too large", d->iwcd_nbest); return JB200_ERR_UNSUPPORTED; }
-  JB_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  JB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) { set_error("device %d is sm_%d%d; libjb200 is built for sm_90a only", device, prop.major, prop.minor); return JB200_ERR_NODEVICE; }
+extern "C" void jb200_gmm_destroy(jb200_gmm *h) {
+  if (!h) return;
+  cudaSetDevice(h->device);
+  cudaFree(h->d_pk); cudaFree(h->d_tiles); cudaFree(h->d_cd_off); cudaFree(h->d_cd_states); cudaFree(h->d_tbl);
+  cudaFree(h->d_feats); cudaFree(h->d_rows);
+  if (h->stream) cudaStreamDestroy(h->stream);
+  delete h;
+}
 
-  jb200_gmm *h = new jb200_gmm();
-  h->device = device; h->mode = mode; h->sm_count = prop.multiProcessorCount;
-  h->S = d->n_states; h->D = d->dim; h->G = d->n_gauss; h->C = d->n_cdsets; h->max_mix = d->max_mix;
-  h->gprune_method = d->gprune_method; h->gprune_num = d->gprune_num;
-  h->iwcd_method = d->iwcd_method; h->iwcd_nbest = d->iwcd_nbest;
-  h->stride = gmm_stride(h->D);
-  h->row_stride = (h->S + h->C + 3) & ~3;
+// the device half of jb200_gmm_create; mixcnt: Gaussians per state, checked against GMM_TILE_GAUSS
+static int gmm_build(jb200_gmm *h, const jb200_gmm_desc *d, const std::vector<int> &mixcnt) {
   JB_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
 
   // pack records
@@ -376,11 +366,6 @@ extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, j
   }
   // tiles: consecutive states, <= GMM_TILE_STATES states and <= GMM_TILE_GAUSS Gaussians
   std::vector<GmmTile> tiles;
-  std::vector<int> mixcnt(h->S);
-  for (int s = 0; s < h->S; s++) {
-    mixcnt[s] = (h->G > 0) ? d->state_off[s + 1] - d->state_off[s] : 0;
-    if (mixcnt[s] > GMM_TILE_GAUSS) { set_error("state %d has %d mixtures (max %d)", s, mixcnt[s], GMM_TILE_GAUSS); delete h; return JB200_ERR_UNSUPPORTED; }
-  }
   for (int s = 0; s < h->S;) {
     GmmTile t{s, 0, (h->G > 0) ? d->state_off[s] : 0, 0};
     while (s < h->S && t.ns < GMM_TILE_STATES && t.ng + mixcnt[s] <= GMM_TILE_GAUSS) { t.ng += mixcnt[s]; t.ns++; s++; }
@@ -407,17 +392,39 @@ extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, j
   build_addlog_table(tbl);
   JB_CUDA(cudaMalloc(&h->d_tbl, tbl.size() * sizeof(float)));
   JB_CUDA(cudaMemcpy(h->d_tbl, tbl.data(), tbl.size() * sizeof(float), cudaMemcpyHostToDevice));
-  *out = h;
   return JB200_OK;
 }
 
-extern "C" void jb200_gmm_destroy(jb200_gmm *h) {
-  if (!h) return;
-  cudaSetDevice(h->device);
-  cudaFree(h->d_pk); cudaFree(h->d_tiles); cudaFree(h->d_cd_off); cudaFree(h->d_cd_states); cudaFree(h->d_tbl);
-  cudaFree(h->d_feats); cudaFree(h->d_rows);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  delete h;
+extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, jb200_gmm **out) {
+  if (!d || !out) { set_error("jb200_gmm_create: null argument"); return JB200_ERR_ARG; }
+  if (d->gprune_method != JB200_GPRUNE_NONE && (d->gprune_num < 1 || d->gprune_num > GMM_NMAX)) {
+    set_error("-tmix %d outside supported range 1..%d", d->gprune_num, GMM_NMAX); return JB200_ERR_UNSUPPORTED;
+  }
+  if (d->iwcd_method == JB200_IWCD_NBEST && d->iwcd_nbest > GMM_NMAX) { set_error("-iwcd1 best %d too large", d->iwcd_nbest); return JB200_ERR_UNSUPPORTED; }
+  std::vector<int> mixcnt(d->n_states);
+  for (int s = 0; s < d->n_states; s++) {
+    mixcnt[s] = (d->n_gauss > 0) ? d->state_off[s + 1] - d->state_off[s] : 0;
+    if (mixcnt[s] > GMM_TILE_GAUSS) { set_error("state %d has %d mixtures (max %d)", s, mixcnt[s], GMM_TILE_GAUSS); return JB200_ERR_UNSUPPORTED; }
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (libjb200 has no CPU fallback)"); return JB200_ERR_NODEVICE; }
+  if (device < 0 || device >= ndev) { set_error("device %d out of range (%d devices)", device, ndev); return JB200_ERR_ARG; }
+  JB_CUDA(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  JB_CUDA(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) { set_error("device %d is sm_%d%d; libjb200 is built for sm_90a only", device, prop.major, prop.minor); return JB200_ERR_NODEVICE; }
+
+  jb200_gmm *h = new jb200_gmm();
+  h->device = device; h->mode = mode; h->sm_count = prop.multiProcessorCount;
+  h->S = d->n_states; h->D = d->dim; h->G = d->n_gauss; h->C = d->n_cdsets; h->max_mix = d->max_mix;
+  h->gprune_method = d->gprune_method; h->gprune_num = d->gprune_num;
+  h->iwcd_method = d->iwcd_method; h->iwcd_nbest = d->iwcd_nbest;
+  h->stride = gmm_stride(h->D);
+  h->row_stride = (h->S + h->C + 3) & ~3;
+  const int rc = gmm_build(h, d, mixcnt);
+  if (rc) { jb200_gmm_destroy(h); return rc; }
+  *out = h;
+  return JB200_OK;
 }
 
 extern "C" int jb200_gmm_score_stride(const jb200_gmm *h) { return h ? h->row_stride : 0; }

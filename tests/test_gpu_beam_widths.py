@@ -32,7 +32,7 @@ def _kernel(ds):
 
 
 def _heap_global(beam, n_start, smem_optin):
-    """jb200_decoder_create's placement rule: the heap-select array goes to global memory when it and the per-survivor
+    """size_cut's placement rule (csrc/beam.cu): the heap-select array goes to global memory when it and the per-survivor
     offsets would take more than half of a block's shared memory"""
     maxt = (max(4 * beam + n_start, 5 * beam) + 64 + 3) & ~3
     return (maxt + 4) * 8 + (beam + 2) * 8 > (smem_optin - 2048) // 2

@@ -102,13 +102,15 @@ def test_product_path_fails_loudly_without_a_device():
 
 def test_dnn_create_refuses_inconsistent_widths():
     """jb200_dnn_create checks the net's widths before it looks for a device: an in_dim other than the first layer's
-    input, an out_dim other than the last layer's output, or a width below 1 is JB200_ERR_ARG, with or without a GPU."""
+    input, an out_dim other than the last layer's output, a layer input other than the previous layer's output, or a
+    width below 1 is JB200_ERR_ARG, with or without a GPU."""
     from util import dnn_blob
     rng = np.random.default_rng(0)
     w0, w1 = rng.standard_normal((8, 5)).astype(np.float32), rng.standard_normal((3, 8)).astype(np.float32)
     good = dnn_blob([w0, w1], [np.zeros(8, np.float32), np.zeros(3, np.float32)], np.zeros(3, np.float32))
     bad = {"in_dim": {"dnn.in_dim": 6}, "out_dim": {"dnn.out_dim": 4}, "zero_width": {"dnn.l0.out": 0, "dnn.l1.in": 0},
-           "zero_in": {"dnn.in_dim": 0, "dnn.l0.in": 0}, "zero_out": {"dnn.out_dim": 0, "dnn.l1.out": 0}}
+           "zero_in": {"dnn.in_dim": 0, "dnn.l0.in": 0}, "zero_out": {"dnn.out_dim": 0, "dnn.l1.out": 0},
+           "chain": {"dnn.l0.out": 9}}
 
     def create(blob):
         h = C.c_void_p()
@@ -122,6 +124,67 @@ def test_dnn_create_refuses_inconsistent_widths():
         blob.update({k: np.array([v], np.int32) for k, v in change.items()})
         assert create(blob) == -1, name                           # JB200_ERR_ARG
     assert create(good) in (0, -3)                               # JB200_OK, or JB200_ERR_NODEVICE without a GPU
+
+
+def test_gmm_create_refuses_unsupported_descriptors():
+    """jb200_gmm_create checks -tmix, -iwcd1 best and the mixtures per state before it looks for a device: each is
+    JB200_ERR_UNSUPPORTED, with or without a GPU."""
+    g = Golden("tiny")
+    too_many_mix = g.blob["gmm.state_off"].copy()
+    too_many_mix[1] = too_many_mix[0] + 65
+
+    def create(blob, **fields):
+        ds = desc.Descriptors(blob)
+        for k, v in fields.items():
+            setattr(ds.gmm, k, v)
+        h = C.c_void_p()
+        rc = capi.lib().jb200_gmm_create(C.byref(ds.gmm), 0, capi.GMM_EXACT, C.byref(h))
+        if h:
+            capi.lib().jb200_gmm_destroy(h)
+        return rc
+
+    assert create(g.blob, gprune_method=1, gprune_num=0) == -4               # -tmix 0 with pruning on
+    assert create(g.blob, iwcd_method=2, iwcd_nbest=17) == -4                # -iwcd1 best 17
+    assert create(dict(g.blob, **{"gmm.state_off": too_many_mix})) == -4     # a state with 65 mixtures
+    assert create(g.blob) in (0, -3)                                         # JB200_OK, or JB200_ERR_NODEVICE without a GPU
+
+
+def test_decoder_create_refuses_bad_trees():
+    """jb200_decoder_create checks the tree before it looks at the acoustic model or the device, so each bad tree gets its
+    own error code even with no acoustic model, with or without a GPU; a good tree then gets JB200_ERR_ARG for the
+    missing model.  The too-many-roots refusal is not covered: it needs a tree with 2^18 roots."""
+    def tree(case, mutate=None, **fields):
+        blob = dict(Golden(case).blob)
+        if mutate:
+            mutate(blob)
+        ds = desc.Descriptors(blob)
+        for k, v in fields.items():
+            setattr(ds.tree, k, v)
+        return ds
+
+    def put(blob, name, i, v):
+        blob["tree." + name] = a = blob["tree." + name].copy()
+        a[i] = v
+
+    cases = {
+        "unknown lm_type": (tree("small_b100", lm_type=7), -4),
+        "grammar on a multipath tree": (tree("small_dfa", multipath=1), -4),
+        "grammar without start nodes": (tree("small_dfa", n_init=0), -1),
+        "grammar with a transparent word": (tree("small_dfa", lambda b: put(b, "is_transparent", 0, 1)), -4),
+        "tree too large": (tree("small_b100", n_nodes=1 << 28), -4),
+        "no head silence": (tree("small_b100", head_silwid=-1), -4),
+        "transparent head silence": (tree("small_b100", lambda b: put(b, "is_transparent", b["tree.head_silwid"][0], 1)), -4),
+        "beam width 0": (tree("small_b100", beam_width=0), -4),
+        "beam width 8001": (tree("small_b100", beam_width=8001), -4),
+        "non-emitting node in a non-multipath tree": (tree("tiny", lambda b: put(b, "outstyle", 0, 255)), -4),
+        "shared root without a factoring value": (tree("small_b100", lambda b: put(b, "scid", b["tree.shared_node"][0], 0)), -1),
+    }
+    for case in ("tiny", "small_b100", "small_dfa"):
+        cases[f"{case} without an acoustic model"] = (tree(case), -1)
+    for name, (ds, want) in cases.items():
+        h = C.c_void_p()
+        assert capi.lib().jb200_decoder_create(C.byref(ds.tree), None, 1, 64, C.byref(h)) == want, name
+        assert not h, name
 
 
 def test_nothing_in_the_product_imports_the_oracle():
