@@ -195,14 +195,16 @@ static inline void jb200_blob_free(jb200_blob *b) {
 /* copies the data */
 static inline void jb200_blob_add(jb200_blob *b, const char *name, int dtype, int64_t count, const void *data) {
   jb200_blob_entry *x;
-  size_t nbytes = (size_t)count * jb200_dtype_size(dtype);
+  size_t nbytes = (size_t)count * jb200_dtype_size(dtype), len = strlen(name);
   if (b->n == b->cap) {
     b->cap = b->cap ? b->cap * 2 : 64;
     b->e = (jb200_blob_entry *)realloc(b->e, sizeof(jb200_blob_entry) * b->cap);
   }
   x = &b->e[b->n++];
+  /* at most 47 characters, zero-padded: the name field always ends in '\0' */
+  if (len > sizeof(x->name) - 1) len = sizeof(x->name) - 1;
   memset(x->name, 0, sizeof(x->name));
-  strncpy(x->name, name, sizeof(x->name) - 1);
+  memcpy(x->name, name, len);
   x->dtype = dtype; x->count = count;
   x->data = malloc(nbytes ? nbytes : 1);
   if (nbytes) memcpy(x->data, data, nbytes);
@@ -297,37 +299,44 @@ static inline float jb200_blob_get_f(const jb200_blob *b, const char *name, floa
 }
 
 /* Fill descriptors from a loaded blob (pointers alias the blob's storage).
- * Return 0 on success, -1 if the section is absent. */
-static inline int jb200_gmm_from_blob(const jb200_blob *b, jb200_gmm_desc *g) {
+ * Return 0 on success, -1 if the section is absent or an array is shorter than its declared dimensions. */
+
+/* Only the state / cd-set layout, for a model without Gaussians (DNN-HMM): dim, the mixture counts and every Gaussian
+ * array stay 0 / NULL.  This is what the beam decoder reads of its scorer. */
+static inline int jb200_cd_gmm_from_blob(const jb200_blob *b, jb200_gmm_desc *g) {
   memset(g, 0, sizeof(*g));
-  if (!jb200_blob_find(b, "gmm.mean")) return -1;
   g->n_states = jb200_blob_get_i(b, "gmm.n_states", 0);
+  g->iwcd_method = jb200_blob_get_i(b, "am.iwcd_method", JB200_IWCD_NBEST);
+  g->iwcd_nbest = jb200_blob_get_i(b, "am.iwcd_nbest", 3);
+  g->n_cdsets = jb200_blob_get_i(b, "am.n_cdsets", 0);
+  g->n_cdset_states = jb200_blob_get_i(b, "am.n_cdset_states", 0);
+  g->cd_off = (const int32_t *)jb200_blob_ptr(b, "am.cd_off", NULL);
+  g->cd_states = (const int32_t *)jb200_blob_ptr(b, "am.cd_states", NULL);
+  if (g->n_states < 0 || g->n_cdsets < 0 || g->n_cdset_states < 0) return -1;
+  if (g->n_cdsets > 0 && (!jb200_blob_has(b, "am.cd_off", JB200_I32, (int64_t)g->n_cdsets + 1) ||
+                          !jb200_blob_has(b, "am.cd_states", JB200_I32, g->n_cdset_states))) return -1;
+  return 0;
+}
+
+static inline int jb200_gmm_from_blob(const jb200_blob *b, jb200_gmm_desc *g) {
+  if (jb200_cd_gmm_from_blob(b, g) != 0 || !jb200_blob_find(b, "gmm.mean")) return -1;
   g->dim = jb200_blob_get_i(b, "gmm.dim", 0);
   g->n_gauss = jb200_blob_get_i(b, "gmm.n_gauss", 0);
   g->max_mix = jb200_blob_get_i(b, "gmm.max_mix", 0);
   g->gprune_method = jb200_blob_get_i(b, "gmm.gprune_method", 0);
   g->gprune_num = jb200_blob_get_i(b, "gmm.gprune_num", 0);
-  g->iwcd_method = jb200_blob_get_i(b, "am.iwcd_method", JB200_IWCD_NBEST);
-  g->iwcd_nbest = jb200_blob_get_i(b, "am.iwcd_nbest", 3);
-  g->n_cdsets = jb200_blob_get_i(b, "am.n_cdsets", 0);
-  g->n_cdset_states = jb200_blob_get_i(b, "am.n_cdset_states", 0);
   g->state_off = (const int32_t *)jb200_blob_ptr(b, "gmm.state_off", NULL);
   g->mean = (const float *)jb200_blob_ptr(b, "gmm.mean", NULL);
   g->ivar = (const float *)jb200_blob_ptr(b, "gmm.ivar", NULL);
   g->gconst = (const float *)jb200_blob_ptr(b, "gmm.gconst", NULL);
   g->lnweight = (const float *)jb200_blob_ptr(b, "gmm.lnweight", NULL);
   g->valid = (const uint8_t *)jb200_blob_ptr(b, "gmm.valid", NULL);
-  g->cd_off = (const int32_t *)jb200_blob_ptr(b, "am.cd_off", NULL);
-  g->cd_states = (const int32_t *)jb200_blob_ptr(b, "am.cd_states", NULL);
-  /* every array must be as long as the declared dimensions say */
-  if (g->n_states < 0 || g->dim < 1 || g->n_gauss < 0 || g->n_cdsets < 0 || g->n_cdset_states < 0) return -1;
+  if (g->dim < 1 || g->n_gauss < 0) return -1;
   if (!jb200_blob_has(b, "gmm.state_off", JB200_I32, (int64_t)g->n_states + 1) ||
       !jb200_blob_has(b, "gmm.mean", JB200_F32, (int64_t)g->n_gauss * g->dim) ||
       !jb200_blob_has(b, "gmm.ivar", JB200_F32, (int64_t)g->n_gauss * g->dim) ||
       !jb200_blob_has(b, "gmm.gconst", JB200_F32, g->n_gauss) || !jb200_blob_has(b, "gmm.lnweight", JB200_F32, g->n_gauss) ||
       !jb200_blob_has(b, "gmm.valid", JB200_U8, g->n_gauss)) return -1;
-  if (g->n_cdsets > 0 && (!jb200_blob_has(b, "am.cd_off", JB200_I32, (int64_t)g->n_cdsets + 1) ||
-                          !jb200_blob_has(b, "am.cd_states", JB200_I32, g->n_cdset_states))) return -1;
   return 0;
 }
 

@@ -15,61 +15,49 @@
  * JB200_ATTACH=calcmix attaches only this hook (no cache fill), JB200_ATTACH=1 the whole-utterance scoring.
  * JB200_GMM_MODE=fast selects the FMA/exact-LSE arithmetic (<=1e-4) instead of the bit-exact one.
  */
-#include <julius/juliuslib.h>
-#include "jb200_model.h"
-#include "jb200_dl.h"
+#include "jb200_host.h"
 
 static jb200_api g_api;
-static jb200_gmm *g_gmm = NULL;
-static jb200_dnn *g_dnn = NULL;
-static jb200_gmm_desc g_gd;
-static jb200_dnn_desc g_dd;
-static float *g_scores = NULL; static size_t g_scores_cap = 0;
+static jb200_scorer g_sc;
+static jb200_rows g_in, g_scores;
 /* calcmix state */
-static float *g_gauss = NULL; static int g_gauss_time = -2; static const int32_t *g_state_off = NULL;
+static float *g_gauss = NULL; static int g_gauss_time = -2;
 
 static void on_pass1_begin(Recog *recog, void *dummy) {
   PROCESS_AM *am = recog->amlist;
   HMMWork *wrk = &(am->hmmwrk);
   HTK_Param *param = am->mfcc->param;
-  int T = param->samplenum, S = wrk->statenum, D, t, rc;
-  float *in;
+  const int T = param->samplenum, S = wrk->statenum, D = g_sc.gd.dim;
+  int t, rc;
+  (void)dummy;
   if (T <= 0 || param->is_outprob) return;
   if (recog->jconf->decodeopt.realtime_flag) {
     jlog("WARNING: jb200: real-time (frame-by-frame) input: the per-utterance GPU scoring is skipped\n");
     return;
   }
-  D = g_dnn ? g_dd.in_dim : g_gd.dim;
   if (param->veclen < D) { jlog("ERROR: jb200: parameter vector shorter than the model's input\n"); return; }
-  if ((size_t)T * S > g_scores_cap) { g_scores_cap = (size_t)T * S; g_scores = (float *)realloc(g_scores, sizeof(float) * g_scores_cap); }
-  /* parvec rows are separate allocations in general: gather into one matrix */
-  in = (float *)malloc(sizeof(float) * (size_t)T * D);
-  for (t = 0; t < T; t++) memcpy(in + (size_t)t * D, param->parvec[t], sizeof(float) * D);
-  rc = g_dnn ? g_api.dnn_score_host(g_dnn, in, T, g_scores) : g_api.gmm_score_host(g_gmm, in, T, g_scores);
-  free(in);
+  if (jb200_rows_reserve(&g_scores, (size_t)T * S) != 0 || jb200_gather(&g_in, param, 0, T, D) != 0) {
+    jlog("ERROR: jb200: out of memory\n");
+    return;
+  }
+  rc = g_sc.dnn ? g_api.dnn_score_host(g_sc.dnn, g_in.x, T, g_scores.x) : g_api.gmm_score_host(g_sc.gmm, g_in.x, T, g_scores.x);
   if (rc != 0) { jlog("ERROR: jb200: GPU scoring failed: %s\n", g_api.last_error()); return; }
   /* make the cache rows exist (outprob_cache_extend is static: outprob.c:116), then overwrite them */
   outprob_state(wrk, T - 1, am->hmminfo->ststart, param);
-  for (t = 0; t < T; t++) memcpy(wrk->outprob_cache[t], g_scores + (size_t)t * S, sizeof(float) * S);
+  for (t = 0; t < T; t++) memcpy(wrk->outprob_cache[t], g_scores.x + (size_t)t * S, sizeof(float) * S);
   wrk->OP_time = -1;          /* force outprob_state() to re-latch its per-frame pointers */
   wrk->OP_last_time = -1;
 }
 
 /* calcmix-only attach: a new utterance must not reuse the last utterance's frame of Gaussian scores */
-static void on_pass1_begin_calcmix(Recog *recog, void *dummy) { g_gauss_time = -2; }
+static void on_pass1_begin_calcmix(Recog *recog, void *dummy) { (void)recog; (void)dummy; g_gauss_time = -2; }
 
 int jb200_attach(Recog *recog, jb200_blob *b) {
-  const char *mode = getenv("JB200_GMM_MODE");
   const char *how = getenv("JB200_ATTACH");
   int rc;
   if (jb200_api_load(&g_api, (void *)&jb200_attach) != 0) return -1;
-  if (jb200_dnn_from_blob(b, &g_dd) == 0) {
-    rc = g_api.dnn_create(&g_dd, 0, &g_dnn);
-  } else {
-    if (jb200_gmm_from_blob(b, &g_gd) != 0) { jlog("ERROR: jb200: no acoustic model in the flattened blob\n"); return -1; }
-    g_state_off = g_gd.state_off;
-    rc = g_api.gmm_create(&g_gd, 0, (mode && strcmp(mode, "fast") == 0) ? JB200_GMM_FAST : JB200_GMM_EXACT, &g_gmm);
-  }
+  rc = jb200_scorer_open(&g_sc, &g_api, b, 0);
+  if (rc > 0) { jlog("ERROR: jb200: no acoustic model in the flattened blob\n"); return -1; }
   if (rc != 0) { jlog("ERROR: jb200: cannot create the GPU scorer: %s\n", g_api.last_error()); return -1; }
   if (how && strcmp(how, "calcmix") == 0) {
     /* only the -gprune jb200 surface: the host keeps calling outprob_state -> calc_mix -> calcmix() */
@@ -78,7 +66,7 @@ int jb200_attach(Recog *recog, jb200_blob *b) {
     return 0;
   }
   callback_add(recog, CALLBACK_EVENT_PASS1_BEGIN, on_pass1_begin, NULL);
-  jlog("STAT: jb200: GPU acoustic scoring attached (%s)\n", g_dnn ? "DNN, tensor cores" : "GMM");
+  jlog("STAT: jb200: GPU acoustic scoring attached (%s)\n", g_sc.dnn ? "DNN, tensor cores" : "GMM");
   return 0;
 }
 
@@ -91,6 +79,7 @@ boolean calcmix_init(HMMWork *wrk) {
   wrk->OP_calced_score = (LOGPROB *)malloc(sizeof(LOGPROB) * wrk->OP_calced_maxnum);
   wrk->OP_calced_id = (int *)malloc(sizeof(int) * wrk->OP_calced_maxnum);
   wrk->OP_gprune_num = wrk->OP_calced_maxnum;
+  if (wrk->OP_calced_score == NULL || wrk->OP_calced_id == NULL) { jlog("ERROR: jb200: out of memory\n"); return FALSE; }
   return TRUE;
 }
 
@@ -98,13 +87,17 @@ void calcmix_free(HMMWork *wrk) { free(wrk->OP_calced_score); free(wrk->OP_calce
 
 void calcmix(HMMWork *wrk, HTK_HMM_Dens **g, int num, int *last_id, int lnum) {
   int i, base;
-  if (g_gmm == NULL) { j_internal_error("jb200 calcmix: the GPU scorer is not attached (set JB200_ATTACH=1)\n"); return; }
-  if (g_gauss == NULL) g_gauss = (float *)malloc(sizeof(float) * (g_gd.n_gauss + 1));
+  (void)g; (void)last_id; (void)lnum;
+  if (g_sc.gmm == NULL) { j_internal_error("jb200 calcmix: the GPU scorer is not attached (set JB200_ATTACH=1)\n"); return; }
+  if (g_gauss == NULL && (g_gauss = (float *)malloc(sizeof(float) * (g_sc.gd.n_gauss + 1))) == NULL) {
+    j_internal_error("jb200 calcmix: out of memory\n");
+    return;
+  }
   if (wrk->OP_time != g_gauss_time) {
-    if (g_api.gmm_gauss_host(g_gmm, wrk->OP_vec, g_gauss) != 0) j_internal_error("jb200 calcmix: %s\n", g_api.last_error());
+    if (g_api.gmm_gauss_host(g_sc.gmm, wrk->OP_vec, g_gauss) != 0) j_internal_error("jb200 calcmix: %s\n", g_api.last_error());
     g_gauss_time = wrk->OP_time;
   }
-  base = g_state_off[wrk->OP_state_id];
+  base = g_sc.gd.state_off[wrk->OP_state_id];
   for (i = 0; i < num; i++) { wrk->OP_calced_score[i] = g_gauss[base + i]; wrk->OP_calced_id[i] = i; }
   wrk->OP_calced_num = num;
 }

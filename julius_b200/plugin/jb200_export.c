@@ -82,7 +82,7 @@ static int flatten_gmm(PROCESS_AM *am, jb200_blob *b) {
   HTK_HMM_INFO *hi = am->hmminfo;
   HTK_HMM_State *st;
   int S = hi->totalstatenum, D = hi->opt.vec_size, G = 0, i, d, m;
-  int *off, *nmix;
+  int *off;
   float *mean, *ivar, *gconst, *lnw;
   unsigned char *valid;
   HTK_HMM_State **byid;

@@ -32,18 +32,26 @@ def _prepare(case, tmp_path):
     return g, d, files
 
 
+def _assert_same_utts(got, want):
+    """a host dump against the golden utterances (or another run's dump): trellis atoms, status, words and fp32 score"""
+    assert len(got) == len(want)
+    for i, (u, ref) in enumerate(zip(got, want)):
+        ok, why = atoms_equal(u.atoms, ref.atoms)
+        assert ok, f"utterance {i}: {why}"
+        assert u.status == ref.status, f"utterance {i}: status {u.status} != {ref.status}"
+        assert u.words == ref.words, f"utterance {i}: words {u.words} != {ref.words}"
+        assert np.float32(u.score) == np.float32(ref.score), f"utterance {i}: score {u.score} != {ref.score}"
+
+
 @pytest.mark.parametrize("case", ["tiny", "small_b100", "small_iwsp"])
 def test_attached_gpu_scores_drive_the_stock_beam(case, tmp_path):
     from oracle import ffi
     g, d, files = _prepare(case, tmp_path)
     dump, out = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], env_extra={"JB200_ATTACH": "1"})
     utts = refdump.load_refdump(dump)
-    assert len(utts) == len(g.utts)
+    _assert_same_utts(utts, g.utts)
     for u, ref in zip(utts, g.utts):
         assert np.array_equal(u.outprob.view(np.uint32), ref.outprob.view(np.uint32))
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
 
 
 @pytest.mark.parametrize("case", ["tiny", "small_b100", "small_safe", "small_mp", "small_iwsp"])
@@ -51,13 +59,7 @@ def test_stock_host_with_gpu_beam_linked_in(case, tmp_path):
     from oracle import ffi
     g, d, files = _prepare(case, tmp_path)
     dump, out = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], binary=ffi.JREF_GPU)
-    utts = refdump.load_refdump(dump)
-    assert len(utts) == len(g.utts)
-    for u, ref in zip(utts, g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.status == ref.status
-        assert u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
+    _assert_same_utts(refdump.load_refdump(dump), g.utts)
 
 
 def _results(out):
@@ -94,12 +96,10 @@ def test_calcmix_hook_equals_gprune_none(tmp_path):
     dump0, _ = ffi.run_ref(d, files, extra_args=["-gprune", "none"], dump="none.jrf")
     dump1, out = ffi.run_ref(d, files, extra_args=["-gprune", "jb200"], dump="hook.jrf", env_extra={"JB200_ATTACH": "calcmix"})
     want, got = refdump.load_refdump(dump0), refdump.load_refdump(dump1)
-    assert len(want) == len(got) == len(files)
+    assert len(want) == len(files)
+    _assert_same_utts(got, want)
     for u, v in zip(want, got):
         assert np.array_equal(u.outprob.view(np.uint32), v.outprob.view(np.uint32))
-        ok, why = atoms_equal(v.atoms, u.atoms)
-        assert ok, why
-        assert u.words == v.words and np.float32(u.score) == np.float32(v.score)
 
 
 def test_beam_shim_decode_ahead_over_a_file_list(tmp_path):
@@ -115,23 +115,19 @@ def test_beam_shim_decode_ahead_over_a_file_list(tmp_path):
         f.write("\n".join(files) + "\n")
     dump, out = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], binary=ffi.JREF_GPU,
                             env_extra={"JB200_FILELIST": lst, "JB200_AHEAD": "3", "JB200_SHIM_VERBOSE": "1"})
-    utts = refdump.load_refdump(dump)
-    assert len(utts) == len(files)
-    for u, ref in zip(utts, g.utts + g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.status == ref.status and u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
+    _assert_same_utts(refdump.load_refdump(dump), g.utts + g.utts)
     assert out.count("from_cache") == len(files)
     assert out.count("JB200_SHIM batch") == (len(files) + 2) // 3
-    # a list that does not match what the host reads is harmless: everything is decoded singly, same result
+    # a list that does not match what the host reads is harmless: the same batches are decoded, but only the utterances
+    # whose file sits at the same place in both lists are answered from them, the others are decoded singly; same result
     bad = os.path.join(d, "bad.lst")
     with open(bad, "w") as f:
         f.write("\n".join(reversed(files)) + "\n")
     dump2, out2 = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], binary=ffi.JREF_GPU, dump="bad.jrf",
                               env_extra={"JB200_FILELIST": bad, "JB200_AHEAD": "3", "JB200_SHIM_VERBOSE": "1"})
-    for u, ref in zip(refdump.load_refdump(dump2), g.utts + g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
+    _assert_same_utts(refdump.load_refdump(dump2), g.utts + g.utts)
+    assert out2.count("from_cache") == sum(a == b for a, b in zip(files, reversed(files)))
+    assert out2.count("JB200_SHIM batch") == (len(files) + 2) // 3
 
 
 @pytest.mark.parametrize("case", ["small_b100", "small_mp"])
@@ -145,13 +141,7 @@ def test_stock_host_drives_the_gpu_beam_frame_by_frame(case, frames, tmp_path):
     g, d, files = _prepare(case, tmp_path)
     dump, out = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], binary=ffi.JREF_GPU,
                             env_extra={"JB200_STREAM": "1", "JB200_STREAM_FRAMES": frames})
-    utts = refdump.load_refdump(dump)
-    assert len(utts) == len(g.utts)
-    for u, ref in zip(utts, g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.status == ref.status
-        assert u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
+    _assert_same_utts(refdump.load_refdump(dump), g.utts)
 
 
 @pytest.mark.parametrize("case", ["small_b100", "small_mp"])
@@ -168,10 +158,7 @@ def test_progressive_output_matches_the_stock_host(case, tmp_path):
     dump, out = ffi.run_ref(d, files, extra_args=extra, binary=ffi.JREF_GPU, env_extra={"JREF_INTERIM": "1"})
     got = [ln for ln in out.splitlines() if ln.startswith("JREF_INTERIM")]
     assert got == want
-    for u, ref in zip(refdump.load_refdump(dump), g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
+    _assert_same_utts(refdump.load_refdump(dump), g.utts)
 
 
 def test_user_defined_lm_through_the_gpu_beam(tmp_path):
@@ -181,12 +168,7 @@ def test_user_defined_lm_through_the_gpu_beam(tmp_path):
     from oracle import ffi
     g, d, files = _prepare("small_userlm", tmp_path)
     dump, out = ffi.run_ref(d, files, extra_args=g.meta["extra_args"], binary=ffi.JREF_GPU, env_extra=g.meta["env"])
-    utts = refdump.load_refdump(dump)
-    assert len(utts) == len(g.utts)
-    for u, ref in zip(utts, g.utts):
-        ok, why = atoms_equal(u.atoms, ref.atoms)
-        assert ok, why
-        assert u.status == ref.status and u.words == ref.words and np.float32(u.score) == np.float32(ref.score)
+    _assert_same_utts(refdump.load_refdump(dump), g.utts)
     # and the user LM really is in effect: the plain N-gram run of the same input scores differently
     plain = Golden("small_b100")
     assert np.float32(plain.utts[0].score) != np.float32(g.utts[0].score)

@@ -85,6 +85,58 @@ def test_descriptor_layouts_match_the_c_header(tmp_path):
         assert [int(x) for x in parts[1:]] == want, parts[0]
 
 
+def test_c_descriptor_readers_match_python(tmp_path):
+    """jb200_gmm_from_blob on a GMM model and jb200_cd_gmm_from_blob (the beam shim's layout-only scorer of a DNN
+    model) read what desc.py reads; a cd-set table shorter than declared is refused; a long entry name is cut to 47
+    characters."""
+    import shutil
+    import subprocess
+    if shutil.which("gcc") is None:
+        pytest.skip("no C compiler")
+    src = r'''#include "jb200_model.h"
+static void show(const char *what, int rc, const jb200_gmm_desc *g) {
+  printf("%s %d %d %d %d %d %d %d %d %d %d\n", what, rc, g->n_states, g->dim, g->n_gauss, g->iwcd_method, g->iwcd_nbest,
+         g->n_cdsets, g->n_cdset_states, g->cd_off ? g->cd_off[g->n_cdsets] : -1, g->mean != NULL);
+}
+int main(int argc, char **argv) {
+  jb200_blob b; jb200_gmm_desc g; jb200_blob_entry *x;
+  if (argc != 3 || jb200_blob_load(&b, argv[1]) != 0) return 1;
+  show("gmm", jb200_gmm_from_blob(&b, &g), &g);
+  jb200_blob_free(&b);
+  if (jb200_blob_load(&b, argv[2]) != 0) return 1;
+  show("cd", jb200_cd_gmm_from_blob(&b, &g), &g);
+  x = (jb200_blob_entry *)jb200_blob_find(&b, "am.cd_off");
+  x->count -= 1;
+  show("short", jb200_cd_gmm_from_blob(&b, &g), &g);
+  jb200_blob_add_i(&b, "LONG", 7);
+  printf("name %s %d\n", b.e[b.n - 1].name, jb200_blob_get_i(&b, "CUT", 0));
+  jb200_blob_free(&b);
+  return 0;
+}
+'''
+    cfile = tmp_path / "readers.c"
+    long_name = "x" * 40 + "_cut_here"
+    cfile.write_text(src.replace("LONG", long_name).replace("CUT", long_name[:47]))
+    exe = str(tmp_path / "readers")
+    subprocess.run(["gcc", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"), "-o", exe, str(cfile)],
+                   check=True)
+    tiny, dnn = Golden("tiny"), Golden("small_dnn")
+    out = subprocess.run([exe, os.path.join(tiny.dir, "model.jb2m"), os.path.join(dnn.dir, "model.jb2m")],
+                         capture_output=True, text=True, check=True).stdout.splitlines()
+    rows = {ln.split()[0]: [int(v) if v.lstrip("-").isdigit() else v for v in ln.split()[1:]] for ln in out}
+
+    def want(g, rc, dim, n_gauss, has_mean):
+        return [rc, g.n_states, dim, n_gauss, g.iwcd_method, g.iwcd_nbest, g.n_cdsets, g.n_cdset_states,
+                int(g.cd_off[g.n_cdsets]), has_mean]
+    g = tiny.ds.gmm
+    assert rows["gmm"] == want(g, 0, g.dim, g.n_gauss, 1)
+    c = dnn.ds.cd_only_gmm()
+    assert c.n_cdsets > 0
+    assert rows["cd"] == want(c, 0, 0, 0, 0)
+    assert rows["short"][0] == -1
+    assert rows["name"] == [long_name[:47], 7]
+
+
 def test_product_path_fails_loudly_without_a_device():
     """No CPU fallback: on a machine without an sm_90 GPU every create call of the C-ABI must return an error (and the
     Python mirror raise), never hand back a handle that computes on the host."""
