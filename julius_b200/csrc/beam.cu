@@ -615,6 +615,34 @@ __device__ __forceinline__ int closed_subtree_size(const int c, const int n, con
   return (width - 1) + max(0, min(n - first + 1, width));
 }
 
+// The relocation pass reads the order in windows of RELOC_WINDOW x 32 keys: the loads of a window are independent, and a
+// scan that passes a whole window without a match costs one load round and RELOC_WINDOW ballots instead of RELOC_WINDOW
+// dependent chunk iterations (the pass runs on one warp while the block waits, so its dependent chain is what it costs).
+constexpr int RELOC_WINDOW = 3;
+// The home pre-order positions of the window keys[base .. base + 32 RELOC_WINDOW), two 16-bit positions per register
+// (chunk c in half c & 1 of pre[c >> 1]); 0xffff for keys past nc and for keys[skip]: no interval [lo, hi) of the n < 65536
+// slots holds it.
+__device__ __forceinline__ void reloc_window_load(const unsigned long long *keys, const int nc, const int base, const int skip, const int lane,
+                                                  unsigned (&pre)[(RELOC_WINDOW + 1) / 2]) {
+#pragma unroll
+  for (int c = 0; c < RELOC_WINDOW; c++) {
+    const int idx = base + 32 * c + lane;
+    const unsigned p = (idx < nc && idx != skip) ? 0xffffu - (unsigned)((keys[idx] >> 16) & 0xffffu) : 0xffffu;
+    if (c & 1) pre[c >> 1] |= p << 16; else pre[c >> 1] = p;
+  }
+}
+// first position >= from of the window (chunk c, lane l = position 32c + l) whose home pre-order position lies in
+// [lo, hi); -1 if none
+__device__ __forceinline__ int reloc_window_first(const unsigned (&pre)[(RELOC_WINDOW + 1) / 2], const int lo, const int hi, const int from, const int lane) {
+#pragma unroll
+  for (int c = 0; c < RELOC_WINDOW; c++) {
+    const int p = (int)((pre[c >> 1] >> (16 * (c & 1))) & 0xffffu);
+    const unsigned b = __ballot_sync(0xffffffffu, p >= lo && p < hi && 32 * c + lane >= from);
+    if (b) return 32 * c + __ffs(b) - 1;
+  }
+  return -1;
+}
+
 // ---- the closed form WITH re-insertions ----------------------------------------------------------------------------
 // While every extraction's s is a loser the heap evolves by pull-ups and
 //   (I)  slot x holds the best remaining element of subtree(x) that no ancestor of x holds,
@@ -632,7 +660,7 @@ __device__ __forceinline__ int closed_subtree_size(const int c, const int n, con
 //   * e's key gets the landing slot's pre-order position and moves to its place in the order (behind this step's root).
 // tools/heapdyn.cpp is the CPU model (closed_dynamic_scan), exact on recorded cuts of real decodes and on random heaps
 // with as few as 8 distinct scores.  One warp; returns 0 on anything unexpected (the caller replays the loop instead).
-__device__ __noinline__ int closed_relocate(unsigned long long *keys, const int nc, const int n, const int need, unsigned *flags, unsigned *multi,
+__device__ __forceinline__ int closed_relocate(unsigned long long *keys, const int nc, const int n, const int need, unsigned *flags, unsigned *multi,
                                             unsigned *pay, const int lane) {
   constexpr unsigned FULL = 0xffffffffu;
   const int H = 31 - __clz(n);
@@ -649,16 +677,13 @@ __device__ __noinline__ int closed_relocate(unsigned long long *keys, const int 
         // --- the occupant of leaf m
         int j = 0, a = 1, lo = 0, hi = n, occ = -1;
         bool gone = false;
-        for (int base = k - 1; base < nc && occ < 0 && !gone; base += 32) {
-          const int idx = base + lane;
-          const unsigned long long key = (idx < nc) ? keys[idx] : 0ull;
-          const int pre = 0xffff - (int)((key >> 16) & 0xffffu);
-          unsigned done = 0u;
+        for (int base = k - 1; base < nc && occ < 0 && !gone; base += 32 * RELOC_WINDOW) {
+          unsigned pre[(RELOC_WINDOW + 1) / 2];
+          reloc_window_load(keys, nc, base, -1, lane, pre);
+          int from = 0;
           while (true) {
-            const bool in = (idx < nc) && pre >= lo && pre < hi && !((done >> lane) & 1u);
-            const unsigned mask = __ballot_sync(FULL, in);
-            if (!mask) break;
-            const int f = __ffs(mask) - 1;
+            const int f = reloc_window_first(pre, lo, hi, from, lane);
+            if (f < 0) break;
             if (j == dm) { occ = base + f; break; }
             // the leaf's own candidate, pulled up to level j: only a loser can be in the leaf now
             if (!is_multi && (int)(pay[(unsigned)keys[base + f] & 0xffffu] >> 16) == m) { gone = true; break; }
@@ -667,7 +692,7 @@ __device__ __noinline__ int closed_relocate(unsigned long long *keys, const int 
             const int lsz = closed_subtree_size(2 * a, n, H);
             if (nxt == 2 * a) { lo = lo + 1; hi = lo + lsz; } else { lo = lo + 1 + lsz; }
             a = nxt;
-            done |= (f >= 31) ? FULL : ((2u << f) - 1u);
+            from = f + 1;
           }
         }
         if (occ >= k) {
@@ -678,25 +703,23 @@ __device__ __noinline__ int closed_relocate(unsigned long long *keys, const int 
           const int msz = m - 1;
           int x = 1; lo = 0; hi = n;
           bool stop = (2 * x > msz);
-          for (int base = k; base < nc && !stop; base += 32) {
-            const int idx = base + lane;
-            const unsigned long long key = (idx < nc) ? keys[idx] : 0ull;
-            const int pre = 0xffff - (int)((key >> 16) & 0xffffu);
-            unsigned done = 0u;
+          for (int base = k; base < nc && !stop; base += 32 * RELOC_WINDOW) {
+            unsigned pre[(RELOC_WINDOW + 1) / 2];
+            reloc_window_load(keys, nc, base, occ, lane, pre);
+            int from = 0;
             while (!stop) {
-              const bool in = (idx < nc) && idx != occ && pre >= lo && pre < hi && !((done >> lane) & 1u);
-              const unsigned mask = __ballot_sync(FULL, in);
-              if (!mask) break;
-              const int f = __ffs(mask) - 1;
-              const unsigned osc = __shfl_sync(FULL, (unsigned)(key >> 32), f);
-              const int opre = __shfl_sync(FULL, pre, f);
+              const int f = reloc_window_first(pre, lo, hi, from, lane);
+              if (f < 0) break;
+              const unsigned long long fk = keys[base + f];
+              const unsigned osc = (unsigned)(fk >> 32);
+              const int opre = 0xffff - (int)((fk >> 16) & 0xffffu);
               if (opre == lo) return 0;                     // an unplaced element whose home is x: cannot happen
               if (esc >= osc) { stop = true; break; }        // e stays at x
               const int lsz = closed_subtree_size(2 * x, n, H);
               if (opre < lo + 1 + lsz) { x = 2 * x; lo = lo + 1; hi = lo + lsz; }
               else { x = 2 * x + 1; lo = lo + 1 + lsz; }
               if (2 * x > msz) { stop = true; break; }
-              done |= (f >= 31) ? FULL : ((2u << f) - 1u);
+              from = f + 1;
             }
           }
           // --- e's home is x (pre-order position lo): new key, new place among the alive elements behind this step's root

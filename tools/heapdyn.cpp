@@ -248,7 +248,7 @@ static bool closed_dynamic_scan(const std::vector<Ent> &H0, int n, int need, flo
   return true;
 }
 
-// ---- lane-by-lane emulation of closed_relocate (csrc/beam.cu): the same chunks, ballots, done masks and shifts ----------
+// ---- lane-by-lane emulation of closed_relocate (csrc/beam.cu): the same windows, ballots and shifts -----------------------
 typedef unsigned long long u64;
 static unsigned fkey_of(float f) { unsigned b; memcpy(&b, &f, 4); return (b & 0x80000000u) ? ~b : (b | 0x80000000u); }
 static int emu_subtree_size(int c, int n, int H) {
@@ -257,6 +257,23 @@ static int emu_subtree_size(int c, int n, int H) {
   const int sh = H - dc;
   const int first = c << sh, width = 1 << sh;
   return (width - 1) + std::max(0, std::min(n - first + 1, width));
+}
+// the scans read the order in windows of EMU_WINDOW chunks of 32 keys (RELOC_WINDOW in beam.cu): lane l of chunk c
+// holds position 32c + l; a ballot per chunk, the first chunk with a match decides
+constexpr int EMU_WINDOW = 3;
+static void emu_window_load(const std::vector<u64> &keys, const int nc, const int base, const int skip, int *pre) {
+  for (int p = 0; p < 32 * EMU_WINDOW; p++) {
+    const int idx = base + p;
+    pre[p] = (idx < nc && idx != skip) ? 0xffff - (int)((keys[idx] >> 16) & 0xffffu) : -1;
+  }
+}
+static int emu_window_first(const int *pre, const int lo, const int hi, const int from) {
+  for (int c = 0; c < EMU_WINDOW; c++) {
+    unsigned b = 0u;
+    for (int lane = 0; lane < 32; lane++) { const int p = 32 * c + lane; if (pre[p] >= lo && pre[p] < hi && p >= from) b |= 1u << lane; }
+    if (b) return 32 * c + __builtin_ffs(b) - 1;
+  }
+  return -1;
 }
 static long g3_chunks = 0, g3_checks = 0, g3_events = 0, g3_frames = 0, g3_ch_occ_event = 0, g3_ch_occ_gone = 0, g3_ch_occ_none = 0, g3_n_gone = 0, g3_n_none = 0, g3_ch_chain = 0, g3_ch_cnt = 0;
 static int emu_relocate(std::vector<u64> &keys, const int nc, const int n, const int need, std::vector<unsigned> &flags, std::vector<unsigned> &multi, std::vector<unsigned> &pay) {
@@ -275,20 +292,14 @@ static int emu_relocate(std::vector<u64> &keys, const int nc, const int n, const
         bool gone = false;
         g3_checks++;
         const long c0 = g3_chunks;
-        for (int base = k - 1; base < nc && occ < 0 && !gone; base += 32) {
-          unsigned done = 0u;
-          g3_chunks++;
+        for (int base = k - 1; base < nc && occ < 0 && !gone; base += 32 * EMU_WINDOW) {
+          int pre[32 * EMU_WINDOW];
+          emu_window_load(keys, nc, base, -1, pre);
+          int from = 0;
+          g3_chunks += std::min(EMU_WINDOW, (nc - base + 31) / 32);     // chunks that hold keys
           while (true) {
-            unsigned mask = 0u;
-            for (int lane = 0; lane < 32; lane++) {
-              const int idx = base + lane;
-              const u64 key = (idx < nc) ? keys[idx] : 0ull;
-              const int pre = 0xffff - (int)((key >> 16) & 0xffffu);
-              const bool in = (idx < nc) && pre >= lo && pre < hi && !((done >> lane) & 1u);
-              if (in) mask |= 1u << lane;
-            }
-            if (!mask) break;
-            const int f = __builtin_ffs(mask) - 1;
+            const int f = emu_window_first(pre, lo, hi, from);
+            if (f < 0) break;
             if (j == dm) { occ = base + f; break; }
             // the leaf's own candidate, pulled up to level j: nothing but a loser can be in the leaf (unless a re-inserted
             // element landed there too)
@@ -298,7 +309,7 @@ static int emu_relocate(std::vector<u64> &keys, const int nc, const int n, const
             const int lsz = emu_subtree_size(2 * a, n, H);
             if (nxt == 2 * a) { lo = lo + 1; hi = lo + lsz; } else { lo = lo + 1 + lsz; }
             a = nxt;
-            done |= (f >= 31) ? 0xffffffffu : ((2u << f) - 1u);
+            from = f + 1;
           }
         }
         if (occ >= k) g3_ch_occ_event += g3_chunks - c0; else if (gone) { g3_ch_occ_gone += g3_chunks - c0; g3_n_gone++; } else { g3_ch_occ_none += g3_chunks - c0; g3_n_none++; }
@@ -310,20 +321,14 @@ static int emu_relocate(std::vector<u64> &keys, const int nc, const int n, const
           const int msz = m - 1;
           int x = 1; lo = 0; hi = n;
           bool stop = (2 * x > msz);
-          for (int base = k; base < nc && !stop; base += 32) {
-            unsigned done = 0u;
-            g3_chunks++;
+          for (int base = k; base < nc && !stop; base += 32 * EMU_WINDOW) {
+            int pre[32 * EMU_WINDOW];
+            emu_window_load(keys, nc, base, occ, pre);
+            int from = 0;
+            g3_chunks += std::min(EMU_WINDOW, (nc - base + 31) / 32);     // chunks that hold keys
             while (!stop) {
-              unsigned mask = 0u;
-              for (int lane = 0; lane < 32; lane++) {
-                const int idx = base + lane;
-                const u64 key = (idx < nc) ? keys[idx] : 0ull;
-                const int pre = 0xffff - (int)((key >> 16) & 0xffffu);
-                const bool in = (idx < nc) && idx != occ && pre >= lo && pre < hi && !((done >> lane) & 1u);
-                if (in) mask |= 1u << lane;
-              }
-              if (!mask) break;
-              const int f = __builtin_ffs(mask) - 1;
+              const int f = emu_window_first(pre, lo, hi, from);
+              if (f < 0) break;
               const u64 fk = keys[base + f];
               const unsigned osc = (unsigned)(fk >> 32);
               const int opre = 0xffff - (int)((fk >> 16) & 0xffffu);
@@ -333,7 +338,7 @@ static int emu_relocate(std::vector<u64> &keys, const int nc, const int n, const
               if (opre < lo + 1 + lsz) { x = 2 * x; lo = lo + 1; hi = lo + lsz; }
               else { x = 2 * x + 1; lo = lo + 1 + lsz; }
               if (2 * x > msz) { stop = true; break; }
-              done |= (f >= 31) ? 0xffffffffu : ((2u << f) - 1u);
+              from = f + 1;
             }
           }
           g3_ch_chain += g3_chunks - c1;
