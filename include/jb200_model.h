@@ -178,36 +178,42 @@ typedef struct {
 typedef struct {
   int32_t n;
   int32_t cap;
+  int32_t failed;            /* 1 once an add ran out of memory: entries are missing */
   jb200_blob_entry *e;
 } jb200_blob;
 
 static inline size_t jb200_dtype_size(int dtype) { return dtype == JB200_U8 ? 1 : 4; }
 
-static inline void jb200_blob_init(jb200_blob *b) { b->n = 0; b->cap = 0; b->e = NULL; }
+static inline void jb200_blob_init(jb200_blob *b) { b->n = 0; b->cap = 0; b->failed = 0; b->e = NULL; }
 
 static inline void jb200_blob_free(jb200_blob *b) {
   int i;
   for (i = 0; i < b->n; i++) free(b->e[i].data);
   free(b->e);
-  b->n = b->cap = 0; b->e = NULL;
+  jb200_blob_init(b);
 }
 
-/* copies the data */
+/* Copies the data; with count 0 nothing is read, so data may be NULL.  When an allocation fails the entry is not added
+ * and b->failed is set, so that a writer of many entries checks once, after the last. */
 static inline void jb200_blob_add(jb200_blob *b, const char *name, int dtype, int64_t count, const void *data) {
   jb200_blob_entry *x;
   size_t nbytes = (size_t)count * jb200_dtype_size(dtype), len = strlen(name);
+  void *copy;
   if (b->n == b->cap) {
-    b->cap = b->cap ? b->cap * 2 : 64;
-    b->e = (jb200_blob_entry *)realloc(b->e, sizeof(jb200_blob_entry) * b->cap);
+    int32_t cap = b->cap ? b->cap * 2 : 64;
+    jb200_blob_entry *e = (jb200_blob_entry *)realloc(b->e, sizeof(jb200_blob_entry) * cap);
+    if (e == NULL) { b->failed = 1; return; }
+    b->e = e; b->cap = cap;
   }
+  if ((copy = malloc(nbytes ? nbytes : 1)) == NULL) { b->failed = 1; return; }
+  if (nbytes) memcpy(copy, data, nbytes);
   x = &b->e[b->n++];
   /* at most 47 characters, zero-padded: the name field always ends in '\0' */
   if (len > sizeof(x->name) - 1) len = sizeof(x->name) - 1;
   memset(x->name, 0, sizeof(x->name));
   memcpy(x->name, name, len);
   x->dtype = dtype; x->count = count;
-  x->data = malloc(nbytes ? nbytes : 1);
-  if (nbytes) memcpy(x->data, data, nbytes);
+  x->data = copy;
 }
 static inline void jb200_blob_add_i(jb200_blob *b, const char *name, int32_t v) { jb200_blob_add(b, name, JB200_I32, 1, &v); }
 static inline void jb200_blob_add_f(jb200_blob *b, const char *name, float v) { jb200_blob_add(b, name, JB200_F32, 1, &v); }
@@ -218,26 +224,23 @@ static inline const jb200_blob_entry *jb200_blob_find(const jb200_blob *b, const
   return NULL;
 }
 
+/* 0, or -1 when the file cannot be opened, a write comes up short (a full disk) or closing it fails */
 static inline int jb200_blob_save(const jb200_blob *b, const char *path) {
   FILE *fp = fopen(path, "wb");
-  int32_t hdr[3]; int i;
+  int32_t hdr[3]; int i, ok;
   static const char zero[16] = {0};
   if (!fp) return -1;
-  fwrite("JB2M", 1, 4, fp);
   hdr[0] = 1; hdr[1] = b->n; hdr[2] = 0;
-  fwrite(hdr, 4, 3, fp);
-  for (i = 0; i < b->n; i++) {
+  ok = fwrite("JB2M", 1, 4, fp) == 4 && fwrite(hdr, 4, 3, fp) == 3;
+  for (i = 0; i < b->n && ok; i++) {
     const jb200_blob_entry *x = &b->e[i];
-    size_t nbytes = (size_t)x->count * jb200_dtype_size(x->dtype);
+    size_t nbytes = (size_t)x->count * jb200_dtype_size(x->dtype), pad = (16 - nbytes % 16) % 16;
     int32_t dt[2]; dt[0] = x->dtype; dt[1] = 0;
-    fwrite(x->name, 1, 48, fp);
-    fwrite(dt, 4, 2, fp);
-    fwrite(&x->count, 8, 1, fp);
-    fwrite(x->data, 1, nbytes, fp);
-    if (nbytes % 16) fwrite(zero, 1, 16 - nbytes % 16, fp);
+    ok = fwrite(x->name, 1, 48, fp) == 48 && fwrite(dt, 4, 2, fp) == 2 && fwrite(&x->count, 8, 1, fp) == 1 &&
+         fwrite(x->data, 1, nbytes, fp) == nbytes && fwrite(zero, 1, pad, fp) == pad;
   }
-  fclose(fp);
-  return 0;
+  if (fclose(fp) != 0) ok = 0;
+  return ok ? 0 : -1;
 }
 
 /* Reads a blob file.  The file is not trusted: dtype must be one of the three known types, every count must fit in

@@ -47,3 +47,23 @@ def make_fixture(preset, outdir: str, n_utts: int = 2, n_frames: int = 200, seed
     dump, out = ffi.run_ref(outdir, files, extra_args=extra_args, export=os.path.join(outdir, "model.jb2m"),
                             tokens=tokens, lm_args=lm_args, env_extra=env_extra)
     return m, files, dump, out
+
+
+def make_dnn_fixture(preset, outdir: str, dnn: dict, n_utts: int = 2, n_frames: int = 150, seed: int = 17,
+                     extra_args: list = ()):
+    """DNN-HMM: the synthetic model's HMMs scored by a seeded DNN (julius_b200.synth.write_dnn with DnnConfig(**dnn));
+    the utterances are random DNN inputs.  Leaves the same files and returns the same tuple as make_fixture()."""
+    cfg = synth.SynthConfig.preset(preset)
+    m = synth.SynthModel(cfg)
+    m.write_all(outdir)
+    dc = synth.DnnConfig(**dnn)
+    synth.write_dnn(outdir, cfg.n_states, dc)
+    rng = np.random.default_rng(seed)
+    files = []
+    for u in range(n_utts):
+        fn = os.path.join(outdir, f"u{u}.mfc")
+        synth.write_htk_param(fn, synth.sample_dnn_input(rng, n_frames, dc.in_dim), parmkind=synth.PARMKIND_USER)
+        files.append(fn)
+    dump, out = ffi.run_ref(outdir, files, extra_args=["-dnnconf", "dnnconf"] + list(extra_args),
+                            export=os.path.join(outdir, "model.jb2m"))
+    return m, files, dump, out

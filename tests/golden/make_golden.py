@@ -68,11 +68,25 @@ DNN_CASES = {
 }
 
 
-def make_sweep(missing_only=False):
+def export_case(name, outdir):
+    """runs the recipe of golden case `name` (CASES or DNN_CASES) in outdir -> (model, files, dump, stdout)"""
+    if name in DNN_CASES:
+        preset, dkw, nu, nf, extra = DNN_CASES[name]
+        return fixtures.make_dnn_fixture(preset, outdir, dkw, n_utts=nu, n_frames=nf, extra_args=extra)
+    preset, nu, nf, nn, extra = CASES[name]
+    return fixtures.make_fixture(preset, outdir, n_utts=nu, n_frames=nf, noise_utts=nn, extra_args=extra,
+                                 grammar=name in GRAMMAR_CASES, env_extra=CASE_ENV.get(name))
+
+
+def sweep_cases():
+    """[(preset, extra args, grammar, make_fixture kwargs)] of every sweep case"""
     from test_oracle_sweep import SWEEP, GRAMMAR_SWEEP
     cases = [(p, e, False, dict(n_utts=2, n_frames=150, noise_utts=1)) for p, e in SWEEP]
-    cases += [("small", e, True, dict(n_utts=2, n_frames=180, noise_utts=1)) for e in GRAMMAR_SWEEP]
-    for preset, extra, grammar, kw in cases:
+    return cases + [("small", e, True, dict(n_utts=2, n_frames=180, noise_utts=1)) for e in GRAMMAR_SWEEP]
+
+
+def make_sweep(missing_only=False):
+    for preset, extra, grammar, kw in sweep_cases():
         if missing_only and os.path.exists(os.path.join(util.SWEEP_DIR, util.sweep_name(preset, extra, grammar) + ".npz")):
             continue
         tmp = tempfile.mkdtemp(prefix="jb200_golden_")
@@ -93,8 +107,7 @@ def main():
         if only and name not in only:
             continue
         tmp = tempfile.mkdtemp(prefix="jb200_golden_")
-        m, files, dump, out = fixtures.make_fixture(preset, tmp, n_utts=nu, n_frames=nf, noise_utts=nn, extra_args=extra,
-                                                    grammar=name in GRAMMAR_CASES, env_extra=CASE_ENV.get(name))
+        m, files, dump, out = export_case(name, tmp)
         dst = os.path.join(HERE, name)
         os.makedirs(dst, exist_ok=True)
         meta = {"preset": preset, "extra_args": extra, "n_utts": len(files), "grammar": name in GRAMMAR_CASES, "env": CASE_ENV.get(name, {}),
@@ -114,18 +127,7 @@ def main():
         if only and name not in only:
             continue
         tmp = tempfile.mkdtemp(prefix="jb200_golden_")
-        cfg = synth.SynthConfig.preset(preset)
-        m = synth.SynthModel(cfg)
-        m.write_all(tmp)
-        dc = synth.DnnConfig(**dkw)
-        synth.write_dnn(tmp, cfg.n_states, dc)
-        rng = np.random.default_rng(17)
-        files = []
-        for u in range(nu):
-            fn = os.path.join(tmp, f"u{u}.mfc")
-            synth.write_htk_param(fn, synth.sample_dnn_input(rng, nf, dc.in_dim), parmkind=synth.PARMKIND_USER)
-            files.append(fn)
-        dump, out = ffi.run_ref(tmp, files, extra_args=["-dnnconf", "dnnconf"] + extra, export=os.path.join(tmp, "model.jb2m"))
+        m, files, dump, out = export_case(name, tmp)
         dst = os.path.join(HERE, name)
         os.makedirs(dst, exist_ok=True)
         shutil.copy(os.path.join(tmp, "model.jb2m"), dst)

@@ -267,6 +267,7 @@ def test_user_lm_export_limits_are_loud(tmp_path):
     with pytest.raises(RuntimeError):
         fixtures.make_fixture("small", d, n_utts=1, n_frames=50, extra_args=["-userlm", "-b", "60"],
                               env_extra={"JREF_USERLM": "1", "JB200_USERLM_MAXWORDS": "100"})
+    assert not os.path.exists(os.path.join(d, "model.jb2m"))
     # within the limit the same call exports (402 words)
     m, files, dump, out = fixtures.make_fixture("small", d, n_utts=1, n_frames=50, extra_args=["-userlm", "-b", "60"],
                                                 env_extra={"JREF_USERLM": "1"})

@@ -56,6 +56,7 @@ def test_tied_mixture_with_history_dependent_pruning_is_refused(tmp_path):
     from oracle import fixtures
     with pytest.raises(RuntimeError):
         fixtures.make_fixture("small_tm", str(tmp_path), n_utts=1, n_frames=50, extra_args=["-b", "60"])
+    assert not (tmp_path / "model.jb2m").exists()
 
 
 @pytest.mark.parametrize("preset,extra", SWEEP, ids=[" ".join([p] + e) for p, e in SWEEP])
