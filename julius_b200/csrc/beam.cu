@@ -634,13 +634,15 @@ __device__ __forceinline__ void reloc_window_load(const unsigned long long *keys
 // first position >= from of the window (chunk c, lane l = position 32c + l) whose home pre-order position lies in
 // [lo, hi); -1 if none
 __device__ __forceinline__ int reloc_window_first(const unsigned (&pre)[(RELOC_WINDOW + 1) / 2], const int lo, const int hi, const int from, const int lane) {
+  // the ballots of the chunks do not depend on each other: all of them, then the first hit
+  int f = -1;
 #pragma unroll
-  for (int c = 0; c < RELOC_WINDOW; c++) {
+  for (int c = RELOC_WINDOW - 1; c >= 0; c--) {
     const int p = (int)((pre[c >> 1] >> (16 * (c & 1))) & 0xffffu);
     const unsigned b = __ballot_sync(0xffffffffu, p >= lo && p < hi && 32 * c + lane >= from);
-    if (b) return 32 * c + __ffs(b) - 1;
+    if (b) f = 32 * c + __ffs(b) - 1;
   }
-  return -1;
+  return f;
 }
 
 // ---- the closed form WITH re-insertions ----------------------------------------------------------------------------
@@ -783,6 +785,42 @@ __device__ __forceinline__ int closed_relocate(unsigned long long *keys, const i
   return 1;
 }
 
+// ---- the bitonic network's stages with partner distance < SORT_TILE, inside a warp --------------------------------------
+// A warp takes a tile of SORT_TILE consecutive keys into registers, key 32 r + l of the tile in register r of lane l (the
+// loads and stores of a warp are consecutive 8-byte words): partner distance 64 and 32 is a compare-exchange between two
+// registers of a lane, 16 … 1 one with lane l ^ j through a shuffle.  One load → stages → store pass and ONE block barrier
+// run every stage (k, j) with k_lo <= k <= k_hi and j < SORT_TILE, where the strided form pays a barrier per stage.
+// Descending where bit k of the key's index is clear, as in the strided stages.  Keys at index >= nc read as 0 (the
+// padding up to np), keys at index >= np do not exist.  All threads call it; ends with the barrier.
+constexpr int SORT_TILE = 128;
+__device__ __forceinline__ void sort_cx(unsigned long long &a, unsigned long long &b, const bool desc) {
+  if (desc ? (a < b) : (a > b)) { const unsigned long long t = a; a = b; b = t; }
+}
+__device__ __forceinline__ void sort_tile_pass(unsigned long long *keys, const int nc, const int np, const int k_lo, const int k_hi) {
+  const int lane = threadIdx.x & 31;
+  for (int i0 = (threadIdx.x >> 5) * SORT_TILE + lane; i0 - lane < np; i0 += (BEAM_THREADS >> 5) * SORT_TILE) {
+    unsigned long long v[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) v[r] = (i0 + 32 * r < nc) ? keys[i0 + 32 * r] : 0ull;
+    for (int k = k_lo; k <= k_hi; k <<= 1) {
+      if (k >= 128) { sort_cx(v[0], v[2], (i0 & k) == 0); sort_cx(v[1], v[3], (i0 & k) == 0); }
+      if (k >= 64) { sort_cx(v[0], v[1], (i0 & k) == 0); sort_cx(v[2], v[3], ((i0 + 64) & k) == 0); }
+      for (int j = min(k >> 1, 16); j > 0; j >>= 1) {
+        const bool low = ((lane & j) == 0);
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+          const unsigned long long o = __shfl_xor_sync(0xffffffffu, v[r], j);
+          const bool keep_max = (low == (((i0 + 32 * r) & k) == 0));
+          if (keep_max == (o > v[r])) v[r] = o;
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 4; r++) if (i0 + 32 * r < np) keys[i0 + 32 * r] = v[r];
+  }
+  __syncthreads();
+}
+
 __device__ int heap_select_closed(unsigned long long *heap, const int n, const int need, const float lose_below, const int maxt,
                                   unsigned long long *keys, const int key_cap, unsigned *pay, const int pay_cap,
                                   int *ordn, int *s_scratch /* [2] shared ints */) {
@@ -812,14 +850,7 @@ __device__ int heap_select_closed(unsigned long long *heap, const int n, const i
     if (is_c) {
       const int ci = base + __popc(m & ((1u << (tid & 31)) - 1u));
       if (ci < cap) {
-        // pre-order position of slot h in the complete tree of n slots
-        int pre = 0, cur = 1;
-        for (int b = (31 - __clz(h)) - 1; b >= 0; b--) {
-          const int bit = (h >> b) & 1;
-          pre += 1 + (bit ? closed_subtree_size(cur * 2, n, H) : 0);
-          cur = cur * 2 + bit;
-        }
-        keys[ci] = ((unsigned long long)fkey(hval(e)) << 32) | ((unsigned long long)(0xffffu - (unsigned)pre) << 16) | (unsigned)ci;
+        keys[ci] = ((unsigned long long)fkey(hval(e)) << 32) | (unsigned)ci;
         pay[ci] = ((unsigned)h << 16) | (unsigned)(e >> 32);
       }
     }
@@ -829,11 +860,26 @@ __device__ int heap_select_closed(unsigned long long *heap, const int n, const i
   int np = 1; while (np < nc) np <<= 1;
   if (nc > cap || np > key_cap || nc < need) return 0;      // uniform: s_scratch[0] is read after the barrier
   const bool can_relocate = have_flags;
-  for (int i = nc + tid; i < np; i += BEAM_THREADS) keys[i] = 0ull;
+  // the pre-order position of each candidate's slot in the complete tree of n slots goes into its key: one candidate per
+  // thread, so that the warps walk the root paths converged (inside the collection loop only the candidates' lanes would).
+  // A level of the path costs 1, and where it turns right the left sibling's subtree (closed_subtree_size of it).
+  for (int ci = tid; ci < nc; ci += BEAM_THREADS) {
+    const int h = (int)(pay[ci] >> 16), d = 31 - __clz(h);
+    int pre = d;
+    for (int b = d - 1; b >= 0; b--) {
+      if ((h >> b) & 1) {
+        const int sh = H - (d - b), width = 1 << sh;
+        pre += (width - 1) + max(0, min(n - ((((h >> b) ^ 1)) << sh) + 1, width));
+      }
+    }
+    keys[ci] |= (unsigned long long)(0xffffu - (unsigned)pre) << 16;
+  }
   __syncthreads();
-  // 2. bitonic sort, descending
-  for (int k = 2; k <= np; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
+  // 2. bitonic sort, descending: the stages inside a tile in one pass per run of them (the first pass also pads
+  //    keys[nc..np) with zeros), the others one strided pass over the keys each
+  sort_tile_pass(keys, nc, np, 2, min(np, SORT_TILE));
+  for (int k = 2 * SORT_TILE; k <= np; k <<= 1) {
+    for (int j = k >> 1; j >= SORT_TILE; j >>= 1) {
       for (int i = tid; i < (np >> 1); i += BEAM_THREADS) {
         const int a = ((i & ~(j - 1)) << 1) | (i & (j - 1)), b = a | j;
         const unsigned long long ka = keys[a], kb = keys[b];
@@ -842,6 +888,7 @@ __device__ int heap_select_closed(unsigned long long *heap, const int n, const i
       }
       __syncthreads();
     }
+    sort_tile_pass(keys, np, np, k, k);
   }
   // 3. the test: which tail candidates may still be in their leaf when it is taken?  If slot p still held e at step
   //    k = n-p+1, the k-1 elements extracted so far and the d = depth(p) elements above p would all be ahead of e, so
