@@ -598,8 +598,8 @@ __device__ void heap_extract_fast(const CutAreas &ca, const int n, const int ext
 // slot holds its original content or an earlier extraction's s, itself a tail content) and when p is taken, at step
 // k = n-p+1, the k-1 elements extracted so far and the d = depth(p) elements on the slots above p are all ahead of e.
 // So if  rank(e) < k + d  for every tail element that ties with another candidate, no re-insertion can matter and the
-// closed form is exact; otherwise the caller replays the loop (heap_extract_fast).  On the 20k-word workload the test
-// passes in 56 % of the frames (tools/heapstat.cpp); tools/heapsim.cpp checks form + test against the plain loop.
+// closed form is exact; otherwise the relocation pass below follows the re-insertions.  tools/beamcut.cpp models
+// collection, sort, test and relocation pass as this function runs them and checks them against the plain loop.
 //
 // All threads call it after heap_build<true>.  Candidates = elements >= lose_below (a lower bound of the need-th largest
 // score); they are sorted with a bitonic network in `keys` (shared memory: the free part of the heap array, slots
@@ -660,8 +660,8 @@ __device__ __forceinline__ int reloc_window_first(const unsigned (&pre)[(RELOC_W
 //     larger child of x (the left one on a tie: that is the order); e stays at x if its score is >= that element's
 //     ("STVAL >= SVAL(child)", beam.c:1362), else the hole moves into the child whose subtree holds that element's home;
 //   * e's key gets the landing slot's pre-order position and moves to its place in the order (behind this step's root).
-// tools/heapdyn.cpp is the CPU model (closed_dynamic_scan), exact on recorded cuts of real decodes and on random heaps
-// with as few as 8 distinct scores.  One warp; returns 0 on anything unexpected (the caller replays the loop instead).
+// tools/beamcut.cpp emulates it lane by lane, exact on recorded cuts of real decodes and on random heaps with as few as
+// 2 distinct scores.  One warp; returns 0 on anything unexpected (the caller replays the loop instead).
 __device__ __forceinline__ int closed_relocate(unsigned long long *keys, const int nc, const int n, const int need, unsigned *flags, unsigned *multi,
                                             unsigned *pay, const int lane) {
   constexpr unsigned FULL = 0xffffffffu;

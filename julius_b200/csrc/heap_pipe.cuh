@@ -21,8 +21,8 @@
 //     `lose_below`, a lower bound of the smallest score that can be extracted) a tail slot holding a loser is never read
 //     for a decision that matters and never becomes a hole, and a loser stays a loser, so those starts -- 97 % of them
 //     on the 20k-word workload -- need no check at all.
-// tools/heapsim.cpp runs exactly this schedule on the CPU against the plain loop (tests/test_heapsim.py).
-// 1613 ticks for 800 extractions out of 2470 on the 20k-word workload (tools/heapstat.cpp on a real decode).
+// tools/beamcut.cpp runs exactly this schedule on the CPU against the plain loop (tests/test_beamcut.py).
+// 1608 ticks for 800 extractions out of ~2430 on the 20k-word workload (tools/beamcut.cpp on a real decode).
 #pragma once
 #include <cuda_runtime.h>
 

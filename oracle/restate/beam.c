@@ -223,7 +223,7 @@ static void sort_token_downward(Beam *b, int neednum, int totalnum) {
 }
 
 /* test tooling: oracle_set_heap_dump(path) makes every beam cut append (totalnum, neednum, scores in token-index
-   order) to a file, so that tools/heapstat.cpp and the heap micro-benchmarks run on the selects of a real decode */
+   order) to a file, so that tools/beamcut.cpp and the heap micro-benchmarks run on the selects of a real decode */
 static FILE *heap_dump_fp = NULL;
 void oracle_set_heap_dump(const char *path) {
   if (heap_dump_fp) { fclose(heap_dump_fp); heap_dump_fp = NULL; }

@@ -1,5 +1,5 @@
 """Test tooling: decode a few synthetic utterances of a workload with the CPU restatement (oracle/) and record
-every beam cut (token count, beam width, scores in token-index order) for tools/heapstat.cpp / tools/heapsim.cpp.
+every beam cut (token count, beam width, scores in token-index order) for `beamcut --dump` (tools/beamcut.cpp).
 
     python tools/dump_heaps.py tri20k /tmp/hd/tri20k.heaps [n_utts] [n_frames]
 """
