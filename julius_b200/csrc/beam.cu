@@ -1174,9 +1174,11 @@ __device__ __forceinline__ jb200_atom trellis_atom(const Tok &tk, const int wid,
 
 // Word-internal candidate k of token tk on node nr (beam_intra_word_core, beam.c:2004-2177): k = 0 the self-loop if there
 // is one, then the arc to nr.next if there is one, then the explicit arcs.  Entering another node that carries a 1-gram
-// factoring id replaces the token's LM term by the node's.  out = the destination node's output.  beam_kernel_mp keeps
-// its own copy of this arc (phase A2), which reads scid alone: keep the two in step.
+// factoring id replaces the token's LM term by the node's.  WITH_OUT: out = the destination node's output, read with
+// scid as one 8-byte load.  The multipath kernel adds no output here and reads scid alone: the paired load made it
+// 1.8 % slower on dnn60k_mp (H100 80GB HBM3, 400 W limit).
 struct IntraArc { int next; float score, lscore; int out; };
+template <bool WITH_OUT>
 __device__ __forceinline__ IntraArc intra_arc(const BeamParams &p, const Tok &tk, const NodeRec &nr, const int k) {
   int next; float pa;
   const int has_self = (nr.self_a != JB200_LOG_ZERO), has_next = (nr.next_a != JB200_LOG_ZERO);
@@ -1187,9 +1189,12 @@ __device__ __forceinline__ IntraArc intra_arc(const BeamParams &p, const Tok &tk
   float lsc = JB200_LOG_ZERO;
   int out_next = nr.out;
   if (next != tk.node) {
-    const int2 so = __ldg(reinterpret_cast<const int2 *>(&p.nodes[next].scid));
-    const int scid = so.x;
-    out_next = so.y;
+    int scid;
+    if constexpr (WITH_OUT) {
+      const int2 so = __ldg(reinterpret_cast<const int2 *>(&p.nodes[next].scid));
+      scid = so.x;
+      out_next = so.y;
+    } else scid = p.nodes[next].scid;
     if (scid != 0) {
       lsc = max_successor_prob(p, tk.cword, scid) * p.lm_weight + p.lm_penalty;
       tmpsum -= tk.lscore;
@@ -1198,6 +1203,117 @@ __device__ __forceinline__ IntraArc intra_arc(const BeamParams &p, const Tok &tk
   }
   if (lsc == JB200_LOG_ZERO) lsc = tk.lscore;
   return IntraArc{next, tmpsum, lsc, out_next};
+}
+
+// the word-internal candidates of a survivor on node nr that passes the score envelope: one per arc
+__device__ __forceinline__ int arc_count(const NodeRec &nr) {
+  return (nr.self_a != JB200_LOG_ZERO) + (nr.next_a != JB200_LOG_ZERO) + nr.arc_n;
+}
+
+// the survivor j < ns whose candidates offs[j] <= c < offs[j+1] include candidate c
+__device__ __forceinline__ int cand_owner(const int *offs, const int ns, const int c) {
+  int lo = 0, hi = ns;
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (offs[mid] <= c) lo = mid; else hi = mid; }
+  return lo;
+}
+
+// Arrival order (create_token numbering, beam.c:1147-1162).  Candidate `local` of source j arrives as seq_no(j, local);
+// the first arrival at a node creates its token, and the best (the first of equals) gives it its content.  A creator
+// sets the bit at its position in arrival order, and the tokens are numbered by the rank of their bits.
+__device__ __forceinline__ unsigned seq_no(const int j, const int local) { return (unsigned)j * SEQ_LOCAL + (unsigned)local; }
+__device__ __forceinline__ bool first_arrival(const SlotView &slots, const int node, const unsigned seq) {
+  return (unsigned)__ldcg(slots.fs(node)) == seq;
+}
+__device__ __forceinline__ unsigned winner_seq(const SlotView &slots, const int node) {
+  return ~(unsigned)(__ldcg(slots.bk(node)) & 0xffffffffu);
+}
+__device__ __forceinline__ void mark_creator(unsigned *bits, const int pos) { atomicOr(bits + (pos >> 5), 1u << (pos & 31)); }
+// wbits = bits[pos >> 5]
+__device__ __forceinline__ int creation_rank(const unsigned wbits, const int *wpre, const int pos) {
+  return wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
+}
+
+// Word end tk on node stend at slot ai of the trellis (save_trellis, beam.c:2209, ending at frame endtime; save = false
+// stores nothing and flags an overflow) and, when the word may be followed (is_tr), cross-word source wi: the survivor j,
+// base = the score the next word starts from (beam.c:2306-2307: plus wordend_a, WORDEND_A, except on multipath trees),
+// and the first isolated-root candidate at nintra.  The best source goes to *webest; beam.c:2308 keeps the FIRST maximum.
+// (wordend_a is read here, not by the caller: read before the branches, it delays the caller's token loads.)
+template <bool WORDEND_A>
+__device__ __forceinline__ void word_end(const BeamParams &p, const UttAreas &ua, const Tok &tk, const int stend,
+                                         const int endtime, const bool save, const int ai, const bool is_tr, const int wi,
+                                         const int j, const int nintra, unsigned long long *webest,
+                                         int *overflow) {
+  if (save && ai < ua.atom_cap) ua.araw[ai] = trellis_atom(tk, stend, endtime, ua.araw);
+  else *overflow = 1;
+  if (!is_tr) return;
+  if (wi < p.maxw && ai < ua.atom_cap) {
+    WEnd w;
+    const int transp = p.is_transp[stend];
+    w.j = j; w.atom = ai; w.last_word = transp ? tk.cword : stend;
+    w.base = tk.score;
+    if constexpr (WORDEND_A) w.base += __ldg(p.wordend_a + stend);
+    w.transp2 = (transp && tk.cword >= 0 && p.is_transp[tk.cword]) ? 1 : 0;
+    w.nintra = nintra;
+    ua.wend[wi] = w;
+    if (w.base > JB200_LOG_ZERO) atomicMax(webest, ((unsigned long long)fkey(w.base) << 32) | (unsigned)(~(unsigned)wi));
+  } else *overflow = 1;
+}
+
+// the score word end w hands to the next word with LM term lsc (beam.c:2430-2442, :2574-2578)
+__device__ __forceinline__ float cross_word_score(const BeamParams &p, const WEnd &w, const float lsc) {
+  float tmpsum = w.base;
+  tmpsum += lsc;
+  if (w.transp2) tmpsum += p.lm_penalty_trans;
+  return tmpsum;
+}
+
+// Cross-word transitions into isolated root col (beam_inter_word, beam.c:2336-2500), pre-reduced over the word ends
+// wend[0..E) in visiting order: the first that reaches it and the best (the first maximum).  ROOT_ARC: a multipath
+// tree's root carries no output, and the candidate lands on a successor of the root through an arc of score pa.
+template <bool GRAMMAR, bool ROOT_ARC>
+__device__ __forceinline__ IsoCand reduce_word_ends(const BeamParams &p, const WEnd *wend, const int E, const int col, const float pa) {
+  float best = JB200_LOG_ZERO, bestl = 0.0f; int beste = -1, firste = -1;
+  for (int e = 0; e < E; e++) {
+    const WEnd w = wend[e];
+    float lsc;
+    if constexpr (GRAMMAR) {
+      // category-pair constraint of (ending word, root's word) and the insertion penalty (beam.c:2404-2411, :2444-2450)
+      if (!__ldg(p.cp_allowed + (size_t)w.last_word * p.n_iso + col)) continue;
+      lsc = p.penalty1 + __ldg(p.cprob + w.last_word);
+    } else {
+      const float tmpprob = __ldg(p.iw + (size_t)w.last_word * p.n_iso + col);
+      lsc = tmpprob * p.lm_weight + p.lm_penalty;
+    }
+    float v = cross_word_score(p, w, lsc);
+    if constexpr (ROOT_ARC) v = v + pa;
+    if (v > JB200_LOG_ZERO) {
+      if (firste < 0) firste = e;
+      if (beste < 0 || best < v) { best = v; beste = e; bestl = lsc; }
+    }
+  }
+  IsoCand ic; ic.score = best; ic.e = beste; ic.lscore = bestl; ic.first_e = firste;
+  return ic;
+}
+
+// 1-gram factoring (beam_inter_word_factoring, beam.c:2549-2616): the score the best word end wb gives shared root i,
+// and in lsc its LM term
+__device__ __forceinline__ float factoring_score(const BeamParams &p, const WEnd &wb, const int i, float &lsc) {
+  lsc = __ldg(p.shared_f + i) * p.lm_weight + p.lm_penalty;
+  return cross_word_score(p, wb, lsc);
+}
+
+// what a token entering the next word from word end w carries of it
+__device__ __forceinline__ void enter_from(Tok &nt, const WEnd &w, const jb200_atom *araw) {
+  nt.tre = w.atom; nt.cword = w.last_word; nt.tre_wid = araw[w.atom].wid;
+}
+
+// init_nodescore, N-gram (beam.c:1631-1665): the frame-0 token on the head silence nr = nodes[head_node], before any output
+__device__ __forceinline__ Tok head_token(const BeamParams &p, const NodeRec &nr) {
+  Tok tk;
+  float ll = (nr.scid != 0) ? max_successor_prob(p, -1, nr.scid) : 0.0f;
+  ll = ll * p.lm_weight + p.lm_penalty;
+  tk.lscore = ll; tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = p.head_node; tk.score = ll;
+  return tk;
 }
 
 // creation order (create_token numbering, beam.c:1147-1162): wpre[w] = the creators marked in bits[0..w); returns their
@@ -1316,13 +1432,9 @@ beam_kernel(const BeamParams p) {
   } else {
   // ================= frame 0: init_nodescore (beam.c:1631-1665) + first sort (:1883) =================
   if (T > 0 && ck_first && tid == 0) {
-    const int node = p.head_node;
-    const NodeRec nr = p.nodes[node];
-    Tok tk;
-    float ll = (nr.scid != 0) ? max_successor_prob(p, -1, nr.scid) : 0.0f;
-    ll = ll * p.lm_weight + p.lm_penalty;
-    tk.lscore = ll; tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = node;
-    tk.score = outprob_style(p, p.rows + (size_t)ck.row_base * p.row_stride, nr.out, -1) + ll;
+    const NodeRec nr = p.nodes[p.head_node];
+    Tok tk = head_token(p, nr);
+    tk.score += outprob_style(p, p.rows + (size_t)ck.row_base * p.row_stride, nr.out, -1);
     ua.tok0[0] = tk;
     ua.surv[0] = tk;
     ua.ord0[0] = 0;
@@ -1366,9 +1478,8 @@ beam_kernel(const BeamParams p) {
         if (j < ns) {
           tk = ua.surv[j];
           nr = p.nodes[tk.node];
-          const bool valid = (tk.score > JB200_LOG_ZERO) && !(tk.score < thr);
-          if (valid) {
-            nin = (nr.self_a != JB200_LOG_ZERO) + (nr.next_a != JB200_LOG_ZERO) + nr.arc_n;
+          if ((tk.score > JB200_LOG_ZERO) && !(tk.score < thr)) {
+            nin = arc_count(nr);
             if (nr.stend >= 0) { is_we = 1; is_tr = (nr.stend != p.tail_silwid); }
           }
         }
@@ -1381,26 +1492,8 @@ beam_kernel(const BeamParams p) {
           // arrival-order position of this survivor's first candidate: its word-internal arcs,
           // then (for a word end that may continue) one slot per isolated root
           poff[j] = carry_c + oc + (carry_w + ow) * p.n_iso;
-          if (is_we) {
-            const int ai = carry_a + oa;
-            if (ai < ua.atom_cap) ua.araw[ai] = trellis_atom(tk, nr.stend, t - 1, ua.araw);
-            else s_overflow = 1;
-            if (is_tr) {
-              const int wi = carry_w + ow;
-              if (wi < MAXW && ai < ua.atom_cap) {
-                WEnd w;
-                const int sword = nr.stend;
-                const int transp = p.is_transp[sword];
-                w.j = j; w.atom = ai; w.last_word = transp ? tk.cword : sword;
-                w.base = tk.score + __ldg(p.wordend_a + sword);
-                w.transp2 = (transp && tk.cword >= 0 && p.is_transp[tk.cword]) ? 1 : 0;
-                w.nintra = nin;
-                ua.wend[wi] = w;
-                if (w.base > JB200_LOG_ZERO)   // beam.c:2308 keeps the FIRST maximum
-                  atomicMax(&s_webest, ((unsigned long long)fkey(w.base) << 32) | (unsigned)(~(unsigned)wi));
-              } else s_overflow = 1;
-            }
-          }
+          if (is_we)
+            word_end<true>(p, ua, tk, nr.stend, t - 1, true, carry_a + oa, is_tr, carry_w + ow, j, nin, &s_webest, &s_overflow);
         }
         carry_c += tot_c; carry_a += tot_a; carry_w += tot_w;
       }
@@ -1420,52 +1513,24 @@ beam_kernel(const BeamParams p) {
     //           candidate (survivors near the tree roots fan out 10-20 ways: per-survivor loops leave most
     //           of the block idle); the owner of candidate c is found by bisection of the offsets
     for (int c = tid; c < cand_total; c += BEAM_THREADS) {
-      int lo = 0, hi = ns;
-      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (offs[mid] <= c) lo = mid; else hi = mid; }
-      const int j = lo;
-      int k = c - offs[j];
+      const int j = cand_owner(offs, ns, c);
+      const int k = c - offs[j];
       const Tok tk = ua.surv[j];
-      const IntraArc ar = intra_arc(p, tk, p.nodes[tk.node], k);
+      const IntraArc ar = intra_arc<true>(p, tk, p.nodes[tk.node], k);
       Cand cd; cd.score = ar.score; cd.node = ar.next; cd.lscore = ar.lscore; cd.src = j;
       ua.cand[c] = cd;
       CandB cb; cb.tre = tk.tre; cb.cword = tk.cword; cb.tre_wid = tk.tre_wid; cb.out = ar.out;
       ua.candb[c] = cb;
-      if (ar.score > JB200_LOG_ZERO) {
-        const unsigned seq = (unsigned)j * SEQ_LOCAL + (unsigned)k;
-        cand_atomics(ua.slots, ar.next, ar.score, seq, seq);
-      }
+      if (ar.score > JB200_LOG_ZERO) cand_atomics(ua.slots, ar.next, ar.score, seq_no(j, k), seq_no(j, k));
     }
     // ---- P2b: cross-word transitions into isolated roots (beam_inter_word, beam.c:2271-2517),
     //           pre-reduced per root over this frame's word ends, visited in survivor order
     for (int i = tid; i < p.n_iso; i += BEAM_THREADS) {
-      const int col = __ldg(p.iso_id + i);
-      float best = JB200_LOG_ZERO, bestl = 0.0f; int beste = -1, firste = -1;
-      for (int e = 0; e < E; e++) {
-        const WEnd w = ua.wend[e];
-        float lsc;
-        if constexpr (GRAMMAR) {
-        // category-pair constraint of (ending word, root's word) and the insertion penalty (beam.c:2404-2411, :2444-2450)
-        if (!__ldg(p.cp_allowed + (size_t)w.last_word * p.n_iso + col)) continue;
-        lsc = p.penalty1 + __ldg(p.cprob + w.last_word);
-        } else {
-        const float tmpprob = __ldg(p.iw + (size_t)w.last_word * p.n_iso + col);
-        lsc = tmpprob * p.lm_weight + p.lm_penalty;
-        }
-        float tmpsum = w.base;
-        tmpsum += lsc;
-        if (w.transp2) tmpsum += p.lm_penalty_trans;
-        if (tmpsum > JB200_LOG_ZERO) {
-          if (firste < 0) firste = e;
-          if (beste < 0 || best < tmpsum) { best = tmpsum; beste = e; bestl = lsc; }
-        }
-      }
-      IsoCand ic; ic.score = best; ic.e = beste; ic.lscore = bestl; ic.first_e = firste;
+      const IsoCand ic = reduce_word_ends<GRAMMAR, false>(p, ua.wend, E, __ldg(p.iso_id + i), 0.0f);
       ua.iso[i] = ic;
-      if (firste >= 0) {
-        const WEnd wf = ua.wend[firste], wb = ua.wend[beste];
-        const unsigned sf = (unsigned)wf.j * SEQ_LOCAL + (unsigned)(wf.nintra + i);
-        const unsigned sw = (unsigned)wb.j * SEQ_LOCAL + (unsigned)(wb.nintra + i);
-        cand_atomics(ua.slots, __ldg(p.iso_node + i), best, sf, sw);
+      if (ic.first_e >= 0) {
+        const WEnd wf = ua.wend[ic.first_e], wb = ua.wend[ic.e];
+        cand_atomics(ua.slots, __ldg(p.iso_node + i), ic.score, seq_no(wf.j, wf.nintra + i), seq_no(wb.j, wb.nintra + i));
       }
     }
     // ---- P2c: best word end -> shared (1-gram factored) roots (beam_inter_word_factoring, :2549-2616)
@@ -1475,15 +1540,10 @@ beam_kernel(const BeamParams p) {
     if (have_we) {
       wbest = ua.wend[(unsigned)(~(unsigned)(webest & 0xffffffffu))];
       for (int i = tid; i < p.n_shared; i += BEAM_THREADS) {
-        const float lsc = __ldg(p.shared_f + i) * p.lm_weight + p.lm_penalty;
-        float tmpsum = wbest.base;
-        tmpsum += lsc;
-        if (wbest.transp2) tmpsum += p.lm_penalty_trans;
+        float lsc;
+        const float tmpsum = factoring_score(p, wbest, i, lsc);
         if (tmpsum < thr) continue;
-        if (tmpsum > JB200_LOG_ZERO) {
-          const unsigned seq = (unsigned)ns * SEQ_LOCAL + (unsigned)i;
-          cand_atomics(ua.slots, __ldg(p.shared_node + i), tmpsum, seq, seq);
-        }
+        if (tmpsum > JB200_LOG_ZERO) cand_atomics(ua.slots, __ldg(p.shared_node + i), tmpsum, seq_no(ns, i), seq_no(ns, i));
       }
     }
     __syncthreads();
@@ -1495,30 +1555,17 @@ beam_kernel(const BeamParams p) {
       const Cand cd = ua.cand[c];
       if (!(cd.score > JB200_LOG_ZERO)) continue;
       const int k = c - offs[cd.src];
-      const unsigned seq = (unsigned)cd.src * SEQ_LOCAL + (unsigned)k;
-      if ((unsigned)__ldcg(ua.slots.fs(cd.node)) == seq) {
-        const int pos = poff[cd.src] + k;
-        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
-      }
+      if (first_arrival(ua.slots, cd.node, seq_no(cd.src, k))) mark_creator(ua.bits, poff[cd.src] + k);
     }
     for (int i = tid; i < p.n_iso; i += BEAM_THREADS) {
       const IsoCand ic = ua.iso[i];
       if (ic.first_e < 0) continue;
       const WEnd wf = ua.wend[ic.first_e];
-      const unsigned seq = (unsigned)wf.j * SEQ_LOCAL + (unsigned)(wf.nintra + i);
-      if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.iso_node + i))) == seq) {
-        const int pos = poff[wf.j] + wf.nintra + i;
-        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
-      }
+      if (first_arrival(ua.slots, __ldg(p.iso_node + i), seq_no(wf.j, wf.nintra + i))) mark_creator(ua.bits, poff[wf.j] + wf.nintra + i);
     }
     if (have_we) {
-      for (int i = tid; i < p.n_shared; i += BEAM_THREADS) {
-        const unsigned seq = (unsigned)ns * SEQ_LOCAL + (unsigned)i;
-        if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.shared_node + i))) == seq) {
-          const int pos = poff[ns] + i;
-          atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
-        }
-      }
+      for (int i = tid; i < p.n_shared; i += BEAM_THREADS)
+        if (first_arrival(ua.slots, __ldg(p.shared_node + i), seq_no(ns, i))) mark_creator(ua.bits, poff[ns] + i);
     }
     __syncthreads();
     PROF_MARK(3);
@@ -1533,18 +1580,14 @@ beam_kernel(const BeamParams p) {
     auto materialise = [&](int pos, int node) {
       const unsigned wbits = __ldcg(ua.bits + (pos >> 5));
       if (!((wbits >> (pos & 31)) & 1u)) return;
-      const int r = ua.wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
-      const unsigned long long bk = __ldcg(ua.slots.bk(node));
-      const unsigned seqw = ~(unsigned)(bk & 0xffffffffu);
+      const int r = creation_rank(wbits, ua.wpre, pos);
+      const unsigned seqw = winner_seq(ua.slots, node);
       const int j = (int)(seqw >> SEQ_LOCAL_BITS), local = (int)(seqw & (SEQ_LOCAL - 1));
       Tok nt; nt.node = node;
       int out;
       if (j == ns) {                                    // factoring pass
-        const float lsc = __ldg(p.shared_f + local) * p.lm_weight + p.lm_penalty;
-        float tmpsum = wbest.base; tmpsum += lsc;
-        if (wbest.transp2) tmpsum += p.lm_penalty_trans;
-        nt.score = tmpsum; nt.lscore = lsc; nt.tre = wbest.atom; nt.cword = wbest.last_word;
-        nt.tre_wid = ua.araw[wbest.atom].wid;
+        nt.score = factoring_score(p, wbest, local, nt.lscore);
+        enter_from(nt, wbest, ua.araw);
         out = p.nodes[node].out;
       } else {
         const int c0 = offs[j], nin = offs[j + 1] - c0;
@@ -1556,8 +1599,8 @@ beam_kernel(const BeamParams p) {
         } else {                                        // isolated-root candidate
           const IsoCand ic = ua.iso[local - nin];
           const WEnd w = ua.wend[ic.e];
-          nt.score = ic.score; nt.lscore = ic.lscore; nt.tre = w.atom; nt.cword = w.last_word;
-          nt.tre_wid = ua.araw[w.atom].wid;
+          nt.score = ic.score; nt.lscore = ic.lscore;
+          enter_from(nt, w, ua.araw);
           out = p.nodes[node].out;
         }
       }
@@ -1704,13 +1747,7 @@ beam_kernel_mp(const BeamParams p) {
 
   // init_nodescore (beam.c:1631-1665): the word-begin node of <s> has no output (:1654-1656)
   if (T > 0 && ck_first && tid == 0) {
-    const int node = p.head_node;
-    const NodeRec nr = p.nodes[node];
-    Tok tk;
-    float ll = (nr.scid != 0) ? max_successor_prob(p, -1, nr.scid) : 0.0f;
-    ll = ll * p.lm_weight + p.lm_penalty;
-    tk.lscore = ll; tk.tre = -1; tk.cword = -1; tk.tre_wid = -1; tk.node = node; tk.score = ll;
-    ua.tok0[0] = tk;
+    ua.tok0[0] = head_token(p, p.nodes[p.head_node]);
     ua.ord0[0] = 0;
     s_ns = 1;
   }
@@ -1749,8 +1786,7 @@ beam_kernel_mp(const BeamParams p) {
         if (j < ns) {
           const Tok tk = tl[ordl[j]];
           const NodeRec nr = p.nodes[tk.node];
-          if ((tk.score > JB200_LOG_ZERO) && !(tk.score < thr))
-            nin = (nr.self_a != JB200_LOG_ZERO) + (nr.next_a != JB200_LOG_ZERO) + nr.arc_n;
+          if ((tk.score > JB200_LOG_ZERO) && !(tk.score < thr)) nin = arc_count(nr);
         }
         int tot_c;
         const int oc = block_excl_scan(nin, s_warp, &tot_c);
@@ -1770,36 +1806,14 @@ beam_kernel_mp(const BeamParams p) {
     //           candidate (survivors near the tree roots fan out 10-20 ways: per-survivor loops leave most
     //           of the block idle); the owner of candidate c is found by bisection of the offsets
     for (int c = tid; c < cand_total; c += BEAM_THREADS) {
-      int lo = 0, hi = ns;
-      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (offs[mid] <= c) lo = mid; else hi = mid; }
-      const int j = lo;
-      int k = c - offs[j];
+      const int j = cand_owner(offs, ns, c);
+      const int k = c - offs[j];
       const Tok tk = tl[ordl[j]];
-      // the arc of intra_arc, kept apart: that one reads (scid, out) as one 8-byte read-only load, which made this
-      // kernel 1.8 % slower on dnn60k_mp (H100 80GB HBM3, 400 W limit); here only scid is needed
       const NodeRec nr = p.nodes[tk.node];
-      int next; float pa;
-      const int has_self = (nr.self_a != JB200_LOG_ZERO), has_next = (nr.next_a != JB200_LOG_ZERO);
-      if (has_self && k == 0) { next = tk.node; pa = nr.self_a; }
-      else if (has_next && k == has_self) { next = nr.next; pa = nr.next_a; }
-      else { const int a = k - has_self - has_next; next = __ldg(p.arc_to + nr.arc_off + a); pa = __ldg(p.arc_a + nr.arc_off + a); }
-      float tmpsum = tk.score + pa;
-      float lsc = JB200_LOG_ZERO;
-      if (next != tk.node) {
-        const int scid = p.nodes[next].scid;
-        if (scid != 0) {
-          lsc = max_successor_prob(p, tk.cword, scid) * p.lm_weight + p.lm_penalty;
-          tmpsum -= tk.lscore;
-          tmpsum += lsc;
-        }
-      }
-      if (lsc == JB200_LOG_ZERO) lsc = tk.lscore;
-      Cand cd; cd.score = tmpsum; cd.node = next; cd.lscore = lsc; cd.src = j;
+      const IntraArc ar = intra_arc<false>(p, tk, nr, k);
+      Cand cd; cd.score = ar.score; cd.node = ar.next; cd.lscore = ar.lscore; cd.src = j;
       ua.cand[c] = cd;
-      if (tmpsum > JB200_LOG_ZERO) {
-        const unsigned seq = (unsigned)j * SEQ_LOCAL + (unsigned)k;
-        cand_atomics(ua.slots, next, tmpsum, seq, seq);
-      }
+      if (ar.score > JB200_LOG_ZERO) cand_atomics(ua.slots, ar.next, ar.score, seq_no(j, k), seq_no(j, k));
     }
     __syncthreads();
     PROF_MARK(2);
@@ -1808,8 +1822,7 @@ beam_kernel_mp(const BeamParams p) {
     for (int c = tid; c < cand_total; c += BEAM_THREADS) {
       const Cand cd = ua.cand[c];
       if (!(cd.score > JB200_LOG_ZERO)) continue;
-      const unsigned seq = (unsigned)cd.src * SEQ_LOCAL + (unsigned)(c - offs[cd.src]);
-      if ((unsigned)__ldcg(ua.slots.fs(cd.node)) == seq) atomicOr(ua.bits + (c >> 5), 1u << (c & 31));
+      if (first_arrival(ua.slots, cd.node, seq_no(cd.src, c - offs[cd.src]))) mark_creator(ua.bits, c);
     }
     __syncthreads();
     PROF_MARK(3);
@@ -1822,10 +1835,9 @@ beam_kernel_mp(const BeamParams p) {
     for (int c = tid; c < cand_total && ncre_a > 0; c += BEAM_THREADS) {
       const unsigned wbits = __ldcg(ua.bits + (c >> 5));
       if (!((wbits >> (c & 31)) & 1u)) continue;
-      const int r = ua.wpre[c >> 5] + __popc(wbits & ((1u << (c & 31)) - 1u));
+      const int r = creation_rank(wbits, ua.wpre, c);
       const int node = ua.cand[c].node;
-      const unsigned long long bk = __ldcg(ua.slots.bk(node));
-      const unsigned seqw = ~(unsigned)(bk & 0xffffffffu);
+      const unsigned seqw = winner_seq(ua.slots, node);
       const int j = (int)(seqw >> SEQ_LOCAL_BITS), local = (int)(seqw & (SEQ_LOCAL - 1));
       const Cand cd = ua.cand[offs[j] + local];
       const Tok src = tl[ordl[j]];
@@ -1872,26 +1884,7 @@ beam_kernel_mp(const BeamParams p) {
         int tot_a, tot_w;
         const int oa = block_excl_scan(is_we, s_warp, &tot_a);
         const int ow = block_excl_scan(is_tr, s_warp, &tot_w);
-        if (is_we) {
-          const int ai = carry_a + oa;
-          if (ai < ua.atom_cap && t > 0) ua.araw[ai] = trellis_atom(tk, nr.stend, t - 1, ua.araw);
-          else s_overflow = 1;
-          if (is_tr) {
-            const int wi = carry_w + ow;
-            if (wi < MAXW && ai < ua.atom_cap) {
-              WEnd w;
-              const int sword = nr.stend;
-              const int transp = p.is_transp[sword];
-              w.j = k; w.atom = ai; w.last_word = transp ? tk.cword : sword;
-              w.base = tk.score;                                   // no wordend_a in multipath (beam.c:2307)
-              w.transp2 = (transp && tk.cword >= 0 && p.is_transp[tk.cword]) ? 1 : 0;
-              w.nintra = 0;
-              ua.wend[wi] = w;
-              if (w.base > JB200_LOG_ZERO)
-                atomicMax(&s_webest, ((unsigned long long)fkey(w.base) << 32) | (unsigned)(~(unsigned)wi));
-            } else s_overflow = 1;
-          }
-        }
+        if (is_we) word_end<false>(p, ua, tk, nr.stend, t - 1, t > 0, carry_a + oa, is_tr, carry_w + ow, k, 0, &s_webest, &s_overflow);
         carry_a += tot_a; carry_w += tot_w;
       }
       if (tid == 0) { s_natoms = min(carry_a, ua.atom_cap); s_E = min(carry_w, MAXW); }
@@ -1909,39 +1902,17 @@ beam_kernel_mp(const BeamParams p) {
     // ---- B2: cross-word transitions through the isolated roots (beam.c:2336-2500), one candidate per
     //          (word end, root successor), pre-reduced per successor over the word ends in visiting order
     for (int ia = tid; ia < p.n_isoarc; ia += BEAM_THREADS) {
-      const int col = __ldg(p.iso_id + __ldg(p.isoarc_iso + ia));
-      const float pa = __ldg(p.isoarc_a + ia);
-      float best = JB200_LOG_ZERO, bestl = 0.0f; int beste = -1, firste = -1;
-      for (int e = 0; e < E; e++) {
-        const WEnd w = ua.wend[e];
-        const float tmpprob = __ldg(p.iw + (size_t)w.last_word * p.n_iso + col);
-        const float lsc = tmpprob * p.lm_weight + p.lm_penalty;
-        float tmpsum = w.base;
-        tmpsum += lsc;
-        if (w.transp2) tmpsum += p.lm_penalty_trans;
-        const float v = tmpsum + pa;
-        if (v > JB200_LOG_ZERO) {
-          if (firste < 0) firste = e;
-          if (beste < 0 || best < v) { best = v; beste = e; bestl = lsc; }
-        }
-      }
-      IsoCand ic; ic.score = best; ic.e = beste; ic.lscore = bestl; ic.first_e = firste;
+      const IsoCand ic = reduce_word_ends<false, true>(p, ua.wend, E, __ldg(p.iso_id + __ldg(p.isoarc_iso + ia)), __ldg(p.isoarc_a + ia));
       ua.iso[ia] = ic;
-      if (firste >= 0) {
-        const unsigned sf = (unsigned)(ua.wend[firste].j + 1) * SEQ_LOCAL + (unsigned)ia;
-        const unsigned sw = (unsigned)(ua.wend[beste].j + 1) * SEQ_LOCAL + (unsigned)ia;
-        cand_atomics(ua.slots, __ldg(p.isoarc_node + ia), best, sf, sw);
-      }
+      if (ic.first_e >= 0)
+        cand_atomics(ua.slots, __ldg(p.isoarc_node + ia), ic.score, seq_no(ua.wend[ic.first_e].j + 1, ia), seq_no(ua.wend[ic.e].j + 1, ia));
     }
     // ---- B3: best word end -> successors of the shared (1-gram factored) roots (beam.c:2549-2616)
     const unsigned long long webest = s_webest;
     const bool have_we = (webest != 0ull) && (nbits_b > 0);
     WEnd wbest; wbest.base = 0.0f; wbest.atom = -1; wbest.last_word = -1; wbest.transp2 = 0; wbest.j = 0; wbest.nintra = 0;
     auto shared_value = [&](int sa, float &lsc, float &v) -> bool {
-      lsc = __ldg(p.shared_f + __ldg(p.sharc_shared + sa)) * p.lm_weight + p.lm_penalty;
-      float tmpsum = wbest.base;
-      tmpsum += lsc;
-      if (wbest.transp2) tmpsum += p.lm_penalty_trans;
+      const float tmpsum = factoring_score(p, wbest, __ldg(p.sharc_shared + sa), lsc);
       if (tmpsum < thr) return false;
       v = tmpsum + __ldg(p.sharc_a + sa);
       return v > JB200_LOG_ZERO;
@@ -1950,9 +1921,7 @@ beam_kernel_mp(const BeamParams p) {
       wbest = ua.wend[(unsigned)(~(unsigned)(webest & 0xffffffffu))];
       for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
         float lsc, v;
-        if (!shared_value(sa, lsc, v)) continue;
-        const unsigned seq = (unsigned)(ns_a + 1) * SEQ_LOCAL + (unsigned)sa;
-        cand_atomics(ua.slots, __ldg(p.sharc_node + sa), v, seq, seq);
+        if (shared_value(sa, lsc, v)) cand_atomics(ua.slots, __ldg(p.sharc_node + sa), v, seq_no(ns_a + 1, sa), seq_no(ns_a + 1, sa));
       }
     }
     __syncthreads();
@@ -1962,20 +1931,12 @@ beam_kernel_mp(const BeamParams p) {
     for (int ia = tid; ia < p.n_isoarc; ia += BEAM_THREADS) {
       const IsoCand ic = ua.iso[ia];
       if (ic.first_e < 0) continue;
-      const unsigned sf = (unsigned)(ua.wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia;
-      if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.isoarc_node + ia))) == sf) {
-        const int pos = ic.first_e * p.n_isoarc + ia;
-        atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
-      }
+      if (first_arrival(ua.slots, __ldg(p.isoarc_node + ia), seq_no(ua.wend[ic.first_e].j + 1, ia)))
+        mark_creator(ua.bits, ic.first_e * p.n_isoarc + ia);
     }
     if (have_we) {
-      for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
-        const unsigned seq = (unsigned)(ns_a + 1) * SEQ_LOCAL + (unsigned)sa;
-        if ((unsigned)__ldcg(ua.slots.fs(__ldg(p.sharc_node + sa))) == seq) {
-          const int pos = E * p.n_isoarc + sa;
-          atomicOr(ua.bits + (pos >> 5), 1u << (pos & 31));
-        }
-      }
+      for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS)
+        if (first_arrival(ua.slots, __ldg(p.sharc_node + sa), seq_no(ns_a + 1, sa))) mark_creator(ua.bits, E * p.n_isoarc + sa);
     }
     __syncthreads();
     PROF_MARK(3);
@@ -1991,24 +1952,25 @@ beam_kernel_mp(const BeamParams p) {
       if (j == ns_a + 1) {
         float lsc, v;
         shared_value(local, lsc, v);
-        nt.score = v; nt.lscore = lsc; nt.tre = wbest.atom; nt.cword = wbest.last_word; nt.tre_wid = ua.araw[wbest.atom].wid;
+        nt.score = v; nt.lscore = lsc;
+        enter_from(nt, wbest, ua.araw);
       } else {
         const IsoCand ic = ua.iso[local];
         const WEnd w = ua.wend[ic.e];
-        nt.score = ic.score; nt.lscore = ic.lscore; nt.tre = w.atom; nt.cword = w.last_word; nt.tre_wid = ua.araw[w.atom].wid;
+        nt.score = ic.score; nt.lscore = ic.lscore;
+        enter_from(nt, w, ua.araw);
       }
     };
     auto settle = [&](int node, unsigned seq_first, unsigned seq_win, int pos) {
       const int fs = __ldcg(ua.slots.fs(node));
-      const unsigned seqw = ~(unsigned)(__ldcg(ua.slots.bk(node)) & 0xffffffffu);
+      const unsigned seqw = winner_seq(ua.slots, node);
       if (fs < 0) {
         if (seqw != seq_win) return;
         Tok nt; nt.node = node;
         winner_content(seqw, nt);
         tn[fs + TOK_EXISTS] = nt;
       } else if ((unsigned)fs == seq_first) {
-        const unsigned wbits = __ldcg(ua.bits + (pos >> 5));
-        const int r = ncre_a + ua.wpre[pos >> 5] + __popc(wbits & ((1u << (pos & 31)) - 1u));
+        const int r = ncre_a + creation_rank(__ldcg(ua.bits + (pos >> 5)), ua.wpre, pos);
         Tok nt; nt.node = node;
         winner_content(seqw, nt);
         tn[r] = nt;
@@ -2018,15 +1980,13 @@ beam_kernel_mp(const BeamParams p) {
       for (int ia = tid; ia < p.n_isoarc; ia += BEAM_THREADS) {
         const IsoCand ic = ua.iso[ia];
         if (ic.first_e < 0) continue;
-        settle(__ldg(p.isoarc_node + ia), (unsigned)(ua.wend[ic.first_e].j + 1) * SEQ_LOCAL + (unsigned)ia,
-               (unsigned)(ua.wend[ic.e].j + 1) * SEQ_LOCAL + (unsigned)ia, ic.first_e * p.n_isoarc + ia);
+        settle(__ldg(p.isoarc_node + ia), seq_no(ua.wend[ic.first_e].j + 1, ia), seq_no(ua.wend[ic.e].j + 1, ia),
+               ic.first_e * p.n_isoarc + ia);
       }
       if (have_we)
         for (int sa = tid; sa < p.n_sharc; sa += BEAM_THREADS) {
           float lsc, v;
-          if (!shared_value(sa, lsc, v)) continue;
-          const unsigned seq = (unsigned)(ns_a + 1) * SEQ_LOCAL + (unsigned)sa;
-          settle(__ldg(p.sharc_node + sa), seq, seq, E * p.n_isoarc + sa);
+          if (shared_value(sa, lsc, v)) settle(__ldg(p.sharc_node + sa), seq_no(ns_a + 1, sa), seq_no(ns_a + 1, sa), E * p.n_isoarc + sa);
         }
     }
     __syncthreads();
