@@ -76,7 +76,8 @@ int jb200_gmm_gauss_host(jb200_gmm *h, const float *feat, float *gauss);
  *   dnn_calc_outprob()   libsent/src/phmm/calc_dnn.c:774-868   (GEMV stack, table logistic,
  *                        log-softmax through addlog_array, minus log10 state prior)
  *   cuda_calc_outprob()  libsent/src/phmm/calc_dnn_cuda.cu:294-321 (the reference's own GPU path)
- * in [T][in_dim] already spliced feature vectors -> scores [T][out_dim], log10.
+ * in [T][in_dim] spliced feature vectors -> scores [T][out_dim], log10; or, after jb200_dnn_set_context, the front-end
+ * frames the vectors are spliced from.
  * Arithmetic: bf16 x3 split products with fp32 accumulation (<= 1e-4 relative, see DESIGN.md).
  * ---------------------------------------------------------------------------------- */
 typedef struct jb200_dnn jb200_dnn;
@@ -84,7 +85,18 @@ int jb200_dnn_create(const jb200_dnn_desc *desc, int device, jb200_dnn **out);
 void jb200_dnn_destroy(jb200_dnn *h);
 int jb200_dnn_in_dim(const jb200_dnn *h);
 int jb200_dnn_out_dim(const jb200_dnn *h);
-int jb200_dnn_score_host(jb200_dnn *h, const float *in, int T, float *scores);
+/* Splice on the device (dnnconf context_len; wav2mfcc.c:160-183, splice_mfcc realtime-1stpass.c:445-460): from now on
+ * every entry point that takes feature vectors for this DNN -- jb200_dnn_score_host, jb200_decode_batch_host/_device
+ * and jb200_stream_feed_host of a decoder it is attached to -- takes frames fl = in_dim / context_len wide, and network
+ * input t is the concatenation of frames t .. t + context_len - 1 of the utterance: N frames give max(0, N - context_len
+ * + 1) decoded frames, the last context_len - 1 frames start no window, and an utterance shorter than context_len decodes
+ * like one of zero frames.  Trellis times, n_frames and interim frame numbers count decoded frames.  The scores are
+ * bit-identical to those of the vectors spliced on the host.  1 (the default) takes spliced vectors.  JB200_ERR_ARG for
+ * context_len < 1, for an in_dim it does not divide, and once the handle has scored frames or been attached to a
+ * decoder.  The score-row entry points (*_scores_host) are unaffected. */
+int jb200_dnn_set_context(jb200_dnn *h, int context_len);
+/* in [n_frames][fl] -> scores [max(0, n_frames - context_len + 1)][out_dim] (context 1: [n_frames][in_dim] -> [n_frames]) */
+int jb200_dnn_score_host(jb200_dnn *h, const float *in, int n_frames, float *scores);
 
 /* ------------------------------------------------------------------------------------
  * Pass-1 decoder (lexicon-tree token passing).  Stands in for
@@ -124,18 +136,23 @@ int jb200_decoder_create(const jb200_tree_desc *tree, jb200_gmm *am, int max_utt
                          jb200_decoder **out);
 void jb200_decoder_destroy(jb200_decoder *d);
 /* DNN-HMM: score frames with `dnn` instead of the GMMs of `am` (am then only carries the state /
- * cd-set layout: a descriptor with n_gauss == 0 is accepted by jb200_gmm_create for this purpose). */
+ * cd-set layout: a descriptor with n_gauss == 0 is accepted by jb200_gmm_create for this purpose).
+ * Fixes the DNN's context length (jb200_dnn_set_context); with context_len > 1 the decoder's feature entry points take
+ * front-end frames. */
 int jb200_decoder_attach_dnn(jb200_decoder *d, jb200_dnn *dnn);
 
 /* End-to-end: host feature vectors -> GPU scoring -> GPU beam -> host results.
  *   feats       [sum T_u][dim]   concatenated utterances (host)
  *   frame_off   [n_utts+1]       utterance boundaries in frames
+ * With a DNN that splices (jb200_dnn_set_context), feats are front-end frames [sum N_u][in_dim / context_len] and
+ * frame_off counts them; utterance u decodes max(0, N_u - context_len + 1) frames, the 32767-frame limit and max_frames
+ * apply to those, and the input frames of a batch may number up to max_frames * context_len.
  * Results stay owned by the decoder until the next call; read them with jb200_decoder_results(). */
 int jb200_decode_batch_host(jb200_decoder *d, const float *feats, const int32_t *frame_off, int n_utts);
 /* Same, but the state-score matrix is given ([sum T_u][n_states], host, log10): used to
  * check the beam in isolation on the reference's own score matrix. */
 int jb200_decode_batch_scores_host(jb200_decoder *d, const float *scores, const int32_t *frame_off, int n_utts);
-/* Device-resident input (bench "value"): d_feats on the decoder's device. */
+/* Device-resident input (bench "value"): d_feats on the decoder's device (front-end frames for a splicing DNN, as above). */
 int jb200_decode_batch_device(jb200_decoder *d, const float *d_feats, const int32_t *frame_off, int n_utts);
 /* copy results of the last batch device->host (called implicitly by the *_host variants) */
 int jb200_decoder_fetch(jb200_decoder *d);
@@ -195,13 +212,18 @@ int jb200_decoder_pipeline_info(jb200_decoder *d, int32_t *n_slices, float *scor
  * utterance (its final frames, possibly none, come with the same call), after which jb200_stream_result() returns what
  * jb200_decoder_results() returns for a batch.  Frame for frame the trellis is identical to the batch decode of the
  * same vectors, whatever the feed sizes.  Per-stream capacity: max_frames / n_streams frames.
+ * With a DNN that splices (jb200_dnn_set_context), feats are front-end frames and n_new[s] counts them: each stream
+ * keeps its last context_len - 1 frames on the device, decodes nothing until context_len frames have arrived and then
+ * one frame per new frame (splice_mfcc, realtime-1stpass.c:445-460), so the trellis is that of the batch decode of the
+ * same frames; an end mark before context_len frames gives the zero-frame result.  frames_done, the capacity and the
+ * interim frame count decoded frames; jb200_stream_open and jb200_stream_restart drop what a stream had kept.
  * ---------------------------------------------------------------------------------- */
 int jb200_stream_open(jb200_decoder *d, int n_streams);          /* all streams at the start of an utterance */
 int jb200_stream_restart(jb200_decoder *d, int stream);          /* one stream starts its next utterance */
 int jb200_stream_feed_host(jb200_decoder *d, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim);
 /* the same on a given state-score matrix ([sum n_new][n_states], host, log10) instead of feature vectors */
 int jb200_stream_feed_scores_host(jb200_decoder *d, const float *scores, const int32_t *n_new, const uint8_t *last, int want_interim);
-/* frames decoded so far; alive = 0 once the beam ran empty (get_back_trellis_proceed's FALSE, beam.c:3012-3015) */
+/* frames decoded so far (decoded, not input, frames for a splicing DNN); alive = 0 once the beam ran empty (get_back_trellis_proceed's FALSE, beam.c:3012-3015) */
 int jb200_stream_status(jb200_decoder *d, int stream, int32_t *frames_done, int32_t *alive, int32_t *ended);
 /* interim result of the last feed that asked for one (want_interim): the best word sequence ending at the last decoded
  * frame, as bt_current_max publishes it in r->result.pass1 (word_num 0 = no word has ended there) */

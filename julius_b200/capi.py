@@ -53,6 +53,7 @@ def lib():
             L.jb200_dnn_in_dim.argtypes = [vp]
             L.jb200_dnn_out_dim.argtypes = [vp]
             L.jb200_dnn_score_host.argtypes = [vp, D.F, C.c_int, D.F]
+            L.jb200_dnn_set_context.argtypes = [vp, C.c_int]
             L.jb200_decoder_attach_dnn.argtypes = [vp, vp]
         if hasattr(L, "jb200_decoder_create"):
             L.jb200_decoder_create.argtypes = [C.POINTER(D.TreeDesc), vp, C.c_int, C.c_int, C.POINTER(vp)]
@@ -166,14 +167,20 @@ class GmmScorer:
 
 
 class DnnScorer:
-    """DNN-HMM forward on the tensor cores (dnn_calc_outprob)."""
+    """DNN-HMM forward on the tensor cores (dnn_calc_outprob).  With context_len > 1 (the dnnconf's context_len) the
+    network input is spliced on the device: score(), and the Decoder it is attached to, take front-end frames
+    in_dim / context_len wide, and N frames give max(0, N - context_len + 1) decoded frames."""
 
-    def __init__(self, ds: D.Descriptors, device: int = 0):
+    def __init__(self, ds: D.Descriptors, device: int = 0, context_len: int = 1):
         self.ds = ds
         self._h = C.c_void_p()
         _check(lib().jb200_dnn_create(C.byref(ds.dnn), device, C.byref(self._h)), "jb200_dnn_create")
         self.in_dim = lib().jb200_dnn_in_dim(self._h)
         self.out_dim = lib().jb200_dnn_out_dim(self._h)
+        if context_len != 1:
+            _check(lib().jb200_dnn_set_context(self._h, context_len), "jb200_dnn_set_context")
+        self.context_len = context_len
+        self.frame_len = self.in_dim // context_len
 
     @property
     def handle(self):
@@ -181,9 +188,9 @@ class DnnScorer:
 
     def score(self, x: np.ndarray) -> np.ndarray:
         x = np.ascontiguousarray(x, np.float32)
-        T = x.shape[0]
-        out = np.empty((T, self.out_dim), np.float32)
-        _check(lib().jb200_dnn_score_host(self._h, _f(x), T, _f(out)), "jb200_dnn_score_host")
+        N = x.shape[0]
+        out = np.empty((max(0, N - self.context_len + 1), self.out_dim), np.float32)
+        _check(lib().jb200_dnn_score_host(self._h, _f(x), N, _f(out)), "jb200_dnn_score_host")
         return out
 
     def close(self):
@@ -219,7 +226,8 @@ class Decoder:
         return off
 
     def decode(self, feats_list):
-        """feats_list: list of [T_u, dim] arrays (host).  Returns list of result dicts."""
+        """feats_list: list of [T_u, dim] arrays (host; front-end frames [N_u, frame_len] when the attached DNN splices).
+        Returns list of result dicts."""
         off = self._offsets([len(x) for x in feats_list])
         cat = np.ascontiguousarray(np.concatenate(feats_list, 0), np.float32)
         _check(lib().jb200_decode_batch_host(self._h, _f(cat), off.ctypes.data_as(D.I), len(feats_list)),

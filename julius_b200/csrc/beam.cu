@@ -40,7 +40,8 @@
 struct jb200_gmm;
 struct jb200_dnn;
 namespace jb200 {
-int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, int row_stride, cudaStream_t st);
+int dnn_fix_context(jb200_dnn *h);
+int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, int row_stride, cudaStream_t st, const SpliceMap &sm);
 int gmm_device(const jb200_gmm *h);
 int gmm_dim(const jb200_gmm *h);
 int gmm_launch_states(jb200_gmm *h, const float *d_feats, int T, float *d_rows, int row_stride, cudaStream_t st,
@@ -2072,6 +2073,17 @@ __global__ void fill_slots_kernel(NodeSlot *slots, size_t n) {
   if (i < n) slots[i] = NodeSlot{0ull, 0x7fffffff, 0};
 }
 
+// Streams of a DNN with a context window (splice_mfcc, realtime-1stpass.c:445-460): after a feed, stream s (block s) keeps
+// the last min(keep, window length) frames of the feed's window -- what it carried plus what came in -- for the windows
+// of its next feed.  Reads the old carry and writes the other buffer of the pair.
+__global__ void carry_update_kernel(const SpliceSeg *__restrict__ seg, const float *__restrict__ in, const float *__restrict__ carry_old,
+                                    float *__restrict__ carry_new, int keep, int fl) {
+  const SpliceSeg s = seg[blockIdx.x];
+  const int n = min(keep, s.n_win), k0 = s.n_win - n;
+  for (int i = threadIdx.x; i < n * fl; i += blockDim.x)
+    carry_new[(size_t)s.carry0 * fl + i] = splice_frame(s, k0 + i / fl, in, carry_old, fl)[i % fl];
+}
+
 }  // namespace jb200
 
 // =============================================================================================
@@ -2119,6 +2131,13 @@ struct jb200_decoder {
   std::vector<int> st_t; std::vector<char> st_started, st_done;
   long long *h_aoff = nullptr;                  // pinned copy of the per-utterance atom offsets
   UttState *h_state = nullptr; int *h_interim_words = nullptr;
+  // a DNN that splices ctx input frames of fl floats into each network input (jb200_dnn_set_context): the segment table
+  // (pinned staging copy and device copy, max_utts + 1 entries), and per stream the input frames of its utterance so far
+  // and its last ctx - 1 of them on the device, in one of a pair of buffers (carry_cur) that a feed's update swaps
+  int ctx = 1, fl = 0;
+  SpliceSeg *h_splice = nullptr, *d_splice = nullptr;
+  float *d_carry[2] = {nullptr, nullptr}; int carry_cur = 0; size_t carry_floats = 0;
+  std::vector<int> st_in;
 };
 
 // from the shared-table arena when it has room, else an allocation of its own
@@ -2587,9 +2606,10 @@ static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index, int interi
   return JB200_OK;
 }
 
-// scores T frames of device features into the score rows, on the main stream
-static int score_frames(jb200_decoder *d, const float *d_feats, int T) {
-  return d->dnn ? dnn_forward_device(d->dnn, d_feats, T, d->d_rows, d->P.row_stride, d->stream)
+// scores T frames of device features into the score rows, on the main stream; a splicing DNN reads its input rows
+// through sm
+static int score_frames(jb200_decoder *d, const float *d_feats, int T, const SpliceMap &sm = SpliceMap()) {
+  return d->dnn ? dnn_forward_device(d->dnn, d_feats, T, d->d_rows, d->P.row_stride, d->stream, sm)
                 : gmm_launch_states(d->am, d_feats, T, d->d_rows, d->P.row_stride, d->stream, nullptr, nullptr, 0);
 }
 
@@ -2672,7 +2692,20 @@ extern "C" int jb200_decoder_attach_dnn(jb200_decoder *d, jb200_dnn *dnn) {
     JB_RC(dev_alloc(d, (size_t)d->max_frames * dim, &nf));
     d->d_feats = nf; d->dim = dim;
   }
-  d->dnn = dnn;
+  // input frames of a splicing DNN are dim / ctx wide: max_frames network inputs' worth of them fit in d_feats as it is
+  const int ctx = dnn_fix_context(dnn), fl = dim / ctx;
+  if (ctx > 1) {
+    if (!d->d_splice) {
+      JB_RC(dev_alloc(d, (size_t)d->max_utts + 1, &d->d_splice));
+      JB_RC(host_alloc(d, (size_t)d->max_utts + 1, &d->h_splice));
+    }
+    const size_t carry = (size_t)d->max_utts * (ctx - 1) * fl;
+    if (carry > d->carry_floats) {
+      for (auto &c : d->d_carry) JB_RC(dev_alloc(d, carry, &c));
+      d->carry_floats = carry;
+    }
+  }
+  d->dnn = dnn; d->ctx = ctx; d->fl = fl;
   return JB200_OK;
 }
 
@@ -2717,14 +2750,45 @@ extern "C" int jb200_decoder_resident_utts(const jb200_decoder *d) { return d ? 
 // What a batch call hands in: features on the device, features on the host, or score rows on the host
 enum BatchInput { FEATS_DEVICE, FEATS_HOST, SCORES_HOST };
 
+// A batch for a splicing DNN: frame_off counts input frames, and utterance u of N_u of them decodes
+// max(0, N_u - ctx + 1) frames (an input shorter than the window decodes none, Julius' "input too short",
+// wav2mfcc.c:132-135).  rows_off gets the offsets of the decoded frames.
+static int splice_rows(jb200_decoder *d, bool host_feats, const int32_t *frame_off, int n_utts, std::vector<int32_t> &rows_off) {
+  if (!frame_off || n_utts < 1) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
+  if (frame_off[0] != 0) { set_error("frame_off[0] must be 0"); return JB200_ERR_ARG; }
+  rows_off.assign(n_utts + 1, 0);
+  for (int u = 0; u < n_utts; u++) {
+    const int N = frame_off[u + 1] - frame_off[u];
+    if (N < 0) { set_error("utterance %d has %d input frames", u, N); return JB200_ERR_ARG; }
+    rows_off[u + 1] = rows_off[u] + std::max(0, N - d->ctx + 1);
+  }
+  if (host_feats && (long long)frame_off[n_utts] * d->fl > (long long)d->max_frames * d->dim) {
+    set_error("batch of %d input frames exceeds decoder capacity %d", frame_off[n_utts], d->max_frames * d->ctx);
+    return JB200_ERR_CAPACITY;
+  }
+  return JB200_OK;
+}
+
 // One batch, ev[0..3] around the upload, the scoring and the beam.  The host variants fetch the results; for device
 // features that is left to jb200_decoder_fetch.  Score rows are never pipelined.
 static int decode_batch(jb200_decoder *d, BatchInput in, const float *x, const int32_t *frame_off, int n_utts) {
   if (in != FEATS_DEVICE && !x) { set_error(in == SCORES_HOST ? "null scores" : "null feats"); return JB200_ERR_ARG; }
-  JB_RC(prepare_batch(d, frame_off, n_utts, in != SCORES_HOST));
+  const bool splice = in != SCORES_HOST && d && d->dnn && d->ctx > 1;
+  std::vector<int32_t> rows_off;
+  if (splice) JB_RC(splice_rows(d, in == FEATS_HOST, frame_off, n_utts, rows_off));
+  JB_RC(prepare_batch(d, splice ? rows_off.data() : frame_off, n_utts, in != SCORES_HOST));
   JB_CUDA(cudaEventRecord(d->ev[0], d->stream));
+  SpliceMap sm;
+  if (splice) {
+    // utterance u's decoded frames read the windows of its own input frames
+    for (int u = 0; u <= n_utts; u++)
+      d->h_splice[u] = SpliceSeg{rows_off[u], frame_off[u], 0, 0, u < n_utts ? frame_off[u + 1] - frame_off[u] : 0};
+    JB_CUDA(cudaMemcpyAsync(d->d_splice, d->h_splice, sizeof(SpliceSeg) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
+    sm.seg = d->d_splice; sm.nseg = n_utts;
+  }
   if (in == FEATS_HOST) {
-    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)d->last_total_frames * d->dim, cudaMemcpyHostToDevice, d->stream));
+    const size_t n = splice ? (size_t)frame_off[n_utts] * d->fl : (size_t)d->last_total_frames * d->dim;
+    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * n, cudaMemcpyHostToDevice, d->stream));
     x = d->d_feats;
   }
   if (in == SCORES_HOST)
@@ -2734,7 +2798,7 @@ static int decode_batch(jb200_decoder *d, BatchInput in, const float *x, const i
   if (d->last_piped) {
     JB_RC(run_pipeline(d, x, n_utts));
   } else {
-    if (in != SCORES_HOST) JB_RC(score_frames(d, x, d->last_total_frames));
+    if (in != SCORES_HOST) JB_RC(score_frames(d, x, d->last_total_frames, sm));
     JB_CUDA(cudaEventRecord(d->ev[2], d->stream));
     JB_RC(launch_beam(d, n_utts, 0));
   }
@@ -2767,7 +2831,7 @@ extern "C" int jb200_stream_open(jb200_decoder *d, int n_streams) {
   const int cap = std::min(d->max_frames / n_streams, 32767);
   if (cap < 1) { set_error("decoder capacity of %d frames is too small for %d streams", d->max_frames, n_streams); return JB200_ERR_CAPACITY; }
   d->stream_mode = true; d->st_n = n_streams; d->st_cap = cap;
-  d->st_t.assign(n_streams, 0); d->st_started.assign(n_streams, 0); d->st_done.assign(n_streams, 0);
+  d->st_t.assign(n_streams, 0); d->st_started.assign(n_streams, 0); d->st_done.assign(n_streams, 0); d->st_in.assign(n_streams, 0);
   std::vector<int32_t> frame_off(n_streams + 1);
   for (int u = 0; u <= n_streams; u++) frame_off[u] = u * cap;
   JB_RC(layout_utts(d, frame_off.data(), n_streams));
@@ -2776,7 +2840,7 @@ extern "C" int jb200_stream_open(jb200_decoder *d, int n_streams) {
   return JB200_OK;
 }
 
-// device part of a feed: rows of the new frames are in d_rows, packed stream-major
+// device part of a feed: rows of the n_new[s] new decoded frames are in d_rows, packed stream-major
 static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t *last, int want_interim) {
   int pack = 0;
   bool any = false, fin_any = false;
@@ -2821,27 +2885,58 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
   return JB200_OK;
 }
 
-// jb200_stream_feed_host / _scores_host: the new frames of every stream, packed stream-major, as features or as score rows
+// jb200_stream_feed_host / _scores_host: the new frames of every stream, packed stream-major, as features or as score rows.
+// For a splicing DNN the features are input frames: stream s's window is the last min(ctx - 1, have) frames it was fed
+// before (have = its input frames so far) followed by its n_new[s] new ones, which give
+// max(0, have + n_new[s] - ctx + 1) - max(0, have - ctx + 1) decoded frames (splice_mfcc: nothing until ctx frames have
+// arrived, then one per frame).
 static int stream_feed(jb200_decoder *d, bool scores, const float *x, const int32_t *n_new, const uint8_t *last, int want_interim) {
   if (!d || !n_new) { set_error("jb200_stream_feed: bad argument"); return JB200_ERR_ARG; }
   if (!d->stream_mode) { set_error("jb200_stream_feed: call jb200_stream_open first"); return JB200_ERR_ARG; }
-  int tot = 0;
+  const bool splice = !scores && d->dnn && d->ctx > 1;
+  std::vector<int32_t> rows(d->st_n);           // decoded frames of each stream in this feed
+  int tot = 0, tot_rows = 0;
   for (int u = 0; u < d->st_n; u++) {
     if (n_new[u] < 0) { set_error("stream %d: negative frame count", u); return JB200_ERR_ARG; }
     if (d->st_done[u] && n_new[u] > 0) { set_error("stream %d has ended; restart it before feeding more frames", u); return JB200_ERR_ARG; }
-    if (d->st_t[u] + n_new[u] > d->st_cap) { set_error("stream %d: %d frames exceed the per-stream capacity %d", u, d->st_t[u] + n_new[u], d->st_cap); return JB200_ERR_CAPACITY; }
-    tot += n_new[u];
+    rows[u] = splice ? std::max(0, d->st_in[u] + n_new[u] - d->ctx + 1) - std::max(0, d->st_in[u] - d->ctx + 1) : n_new[u];
+    if (d->st_t[u] + rows[u] > d->st_cap) { set_error("stream %d: %d frames exceed the per-stream capacity %d", u, d->st_t[u] + rows[u], d->st_cap); return JB200_ERR_CAPACITY; }
+    tot += n_new[u]; tot_rows += rows[u];
   }
-  if (tot > d->max_frames) { set_error("%d new frames exceed decoder capacity %d", tot, d->max_frames); return JB200_ERR_CAPACITY; }
+  if (tot_rows > d->max_frames) { set_error("%d new frames exceed decoder capacity %d", tot_rows, d->max_frames); return JB200_ERR_CAPACITY; }
+  if (splice && (long long)tot * d->fl > (long long)d->max_frames * d->dim) {
+    set_error("%d new input frames exceed decoder capacity %d", tot, d->max_frames * d->ctx);
+    return JB200_ERR_CAPACITY;
+  }
   if (tot > 0 && !x) { set_error(scores ? "null scores" : "null feats"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
   if (tot > 0 && scores)
     JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->P.row_stride, x, sizeof(float) * d->S, sizeof(float) * d->S, tot, cudaMemcpyHostToDevice, d->stream));
-  else if (tot > 0) {
+  else if (tot > 0 && !splice) {
     JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)tot * d->dim, cudaMemcpyHostToDevice, d->stream));
     JB_RC(score_frames(d, d->d_feats, tot));
+  } else if (tot > 0) {
+    JB_CUDA(cudaStreamSynchronize(d->stream));   // the staging segment table may still feed the last feed's copy
+    int pack_in = 0, pack_rows = 0;
+    for (int u = 0; u < d->st_n; u++) {
+      const int have = std::min(d->ctx - 1, d->st_in[u]);
+      d->h_splice[u] = SpliceSeg{pack_rows, pack_in, u * (d->ctx - 1), have, have + n_new[u]};
+      pack_in += n_new[u]; pack_rows += rows[u];
+    }
+    d->h_splice[d->st_n] = SpliceSeg{pack_rows, pack_in, 0, 0, 0};
+    JB_CUDA(cudaMemcpyAsync(d->d_splice, d->h_splice, sizeof(SpliceSeg) * (d->st_n + 1), cudaMemcpyHostToDevice, d->stream));
+    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)tot * d->fl, cudaMemcpyHostToDevice, d->stream));
+    SpliceMap sm;
+    sm.seg = d->d_splice; sm.nseg = d->st_n; sm.carry = d->d_carry[d->carry_cur];
+    JB_RC(score_frames(d, d->d_feats, tot_rows, sm));
+    // after the scoring has read the carry, in stream order: the new carry goes to the other buffer
+    carry_update_kernel<<<d->st_n, 128, 0, d->stream>>>(d->d_splice, d->d_feats, d->d_carry[d->carry_cur], d->d_carry[d->carry_cur ^ 1],
+                                                        d->ctx - 1, d->fl);
+    JB_LAUNCH_CHECK();
+    d->carry_cur ^= 1;
+    for (int u = 0; u < d->st_n; u++) d->st_in[u] += n_new[u];
   }
-  return stream_advance(d, n_new, last, want_interim);
+  return stream_advance(d, rows.data(), last, want_interim);
 }
 
 extern "C" int jb200_stream_feed_host(jb200_decoder *d, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim) {
@@ -2859,7 +2954,7 @@ extern "C" int jb200_stream_restart(jb200_decoder *d, int stream) {
     JB_RC(reset_slots(d, stream, 1));
     JB_CUDA(cudaStreamSynchronize(d->stream));
   }
-  d->st_t[stream] = 0; d->st_started[stream] = 0; d->st_done[stream] = 0;
+  d->st_t[stream] = 0; d->st_started[stream] = 0; d->st_done[stream] = 0; d->st_in[stream] = 0;
   return JB200_OK;
 }
 

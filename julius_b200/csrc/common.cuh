@@ -28,6 +28,23 @@ __device__ __forceinline__ float addlog_step_exact(float y, float x, const float
   return __fadd_rn(y, __ldg(tbl + idx));
 }
 
+// ---- DNN input splicing (wav2mfcc.c:160-183, splice_mfcc realtime-1stpass.c:445-460) -------------------------------
+// A DNN with context_len ctx > 1 takes frames fl = in_dim / ctx wide; network input row r is the concatenation of ctx
+// consecutive frames of a window.  A segment is an utterance of a batch or a stream's feed: its rows start at row0, and
+// its window is n_carry frames carried over from earlier feeds (carry[carry0 ..]) followed by its new frames
+// (in[frame0 ..]), n_win frames in all.  Row r of the segment reads window frames k = r - row0 .. r - row0 + ctx - 1.
+// A table of nseg segments ends with a sentinel whose row0 is the total row count.
+struct SpliceSeg { int row0, frame0, carry0, n_carry, n_win; };
+struct SpliceMap {
+  const SpliceSeg *seg = nullptr;   // device, nseg + 1 entries; nseg == 0: row r is the window in[r .. r + ctx - 1]
+  int nseg = 0;
+  const float *carry = nullptr;     // device [.][fl]
+};
+// frame k of segment s's window
+__device__ __forceinline__ const float *splice_frame(const SpliceSeg &s, int k, const float *in, const float *carry, int fl) {
+  return (k < s.n_carry) ? carry + (size_t)(s.carry0 + k) * fl : in + (size_t)(s.frame0 + k - s.n_carry) * fl;
+}
+
 #define JB_CUDA(expr)                                                              \
   do {                                                                             \
     cudaError_t _e = (expr);                                                       \

@@ -195,12 +195,29 @@ dnn_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   }
 }
 
-// fp32 [M][K] -> bf16 hi/lo [M][ld] (zero padded)
-__global__ void split_bf16_kernel(const float *__restrict__ src, int M, int K, __nv_bfloat16 *hi, __nv_bfloat16 *lo, int ld) {
+// Layer 0's operand: network input rows [M][K] as bf16 hi/lo [M][ld] (zero padded).  Input row r, column c is column
+// c % fl of frame c / fl of row r's window (SpliceSeg), so the operand is bit for bit that of the rows spliced on the
+// host.  Without a segment table the window of row r is src frames r .. r + K / fl - 1, which lie back to back: column c
+// is src[r * fl + c] (with context 1, fl == K, the plain row-major copy).
+__global__ void split_bf16_kernel(const float *__restrict__ src, int fl, const SpliceMap sm, int M, int K, __nv_bfloat16 *hi,
+                                  __nv_bfloat16 *lo, int ld) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (size_t)M * ld) return;
   const int r = (int)(idx / ld), c = (int)(idx % ld);
-  const float v = (c < K) ? src[(size_t)r * K + c] : 0.0f;
+  float v = 0.0f;
+  if (c < K) {
+    if (sm.nseg == 0) {
+      v = src[(size_t)r * fl + c];
+    } else {
+      int a = 0, b = sm.nseg - 1;                              // the last segment whose rows start at or before r
+      while (a < b) {
+        const int m = (a + b + 1) >> 1;
+        if (__ldg(&sm.seg[m].row0) <= r) a = m; else b = m - 1;
+      }
+      const SpliceSeg s = sm.seg[a];
+      v = __ldg(splice_frame(s, r - s.row0 + c / fl, src, sm.carry, fl) + c % fl);
+    }
+  }
   const __nv_bfloat16 h = __float2bfloat16_rn(v);
   hi[idx] = h;
   lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
@@ -260,6 +277,9 @@ struct DnnLayerDev {
 
 struct jb200_dnn {
   int device = 0, n_layers = 0, in_dim = 0, out_dim = 0, row_stride = 0;
+  // input frames are frame_len = in_dim / context wide, spliced context at a time (jb200_dnn_set_context); fixed once
+  // the handle has scored frames or been attached to a decoder
+  int context = 1, frame_len = 0; bool layout_fixed = false;
   std::vector<DnnLayerDev> L;
   float *d_prior = nullptr, *d_logistic = nullptr, *d_addlog = nullptr;
   PFN_encodeTiled encode = nullptr;
@@ -360,7 +380,7 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
   JB_CUDA(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) { set_error("device is sm_%d%d; the wgmma GEMM needs sm_90a", prop.major, prop.minor); return JB200_ERR_NODEVICE; }
   jb200_dnn *h = new jb200_dnn();
-  h->device = device; h->n_layers = d->n_layers; h->in_dim = d->in_dim; h->out_dim = d->out_dim;
+  h->device = device; h->n_layers = d->n_layers; h->in_dim = d->in_dim; h->out_dim = d->out_dim; h->frame_len = d->in_dim;
   h->row_stride = (d->out_dim + 3) & ~3;
   h->n_sm = prop.multiProcessorCount;
   const int rc = dnn_build(h, d);
@@ -371,6 +391,14 @@ extern "C" int jb200_dnn_create(const jb200_dnn_desc *d, int device, jb200_dnn *
 
 extern "C" int jb200_dnn_out_dim(const jb200_dnn *h) { return h ? h->out_dim : 0; }
 extern "C" int jb200_dnn_in_dim(const jb200_dnn *h) { return h ? h->in_dim : 0; }
+
+extern "C" int jb200_dnn_set_context(jb200_dnn *h, int context_len) {
+  if (!h || context_len < 1) { set_error("jb200_dnn_set_context: bad argument"); return JB200_ERR_ARG; }
+  if (h->in_dim % context_len) { set_error("jb200_dnn_set_context: input width %d is not a multiple of %d frames", h->in_dim, context_len); return JB200_ERR_ARG; }
+  if (h->layout_fixed) { set_error("jb200_dnn_set_context: the handle has scored frames or been attached to a decoder"); return JB200_ERR_ARG; }
+  h->context = context_len; h->frame_len = h->in_dim / context_len;
+  return JB200_OK;
+}
 
 static int dnn_reserve(jb200_dnn *h, int T) {
   if (T <= h->cap_frames) return JB200_OK;
@@ -389,8 +417,15 @@ static int dnn_reserve(jb200_dnn *h, int T) {
 }
 
 namespace jb200 {
-// d_in [T][in_dim] fp32 on device -> d_rows [T][row_stride] log10 pseudo-likelihoods
-int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, int row_stride, cudaStream_t st) {
+// the decoder's view of the handle: from now on its input layout stays as it is; returns the context length
+int dnn_fix_context(jb200_dnn *h) {
+  h->layout_fixed = true;
+  return h->context;
+}
+
+// T network input rows, each the window of context frames (frame_len floats each) that sm gives for it, from d_in
+// (fp32, device) -> d_rows [T][row_stride] log10 pseudo-likelihoods
+int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, int row_stride, cudaStream_t st, const SpliceMap &sm) {
   if (T <= 0) return JB200_OK;
   JB_CUDA(cudaSetDevice(h->device));
   int rc = dnn_reserve(h, T); if (rc) return rc;
@@ -398,7 +433,7 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
   {
     const int ld = h->L[0].ld_in;
     const size_t tot = (size_t)T * ld;
-    split_bf16_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(d_in, T, h->in_dim, h->act_hi[0], h->act_lo[0], ld);
+    split_bf16_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(d_in, h->frame_len, sm, T, h->in_dim, h->act_hi[0], h->act_lo[0], ld);
     JB_LAUNCH_CHECK();
   }
   for (int l = 0; l < h->n_layers; l++) {
@@ -424,13 +459,17 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
 }
 }  // namespace jb200
 
-extern "C" int jb200_dnn_score_host(jb200_dnn *h, const float *in, int T, float *scores) {
+// n_frames input frames give n_frames - context + 1 rows (none when the input is shorter than the window); the input
+// copy, (T + context - 1) * frame_len floats, fits in the T * in_dim that dnn_reserve gives d_in
+extern "C" int jb200_dnn_score_host(jb200_dnn *h, const float *in, int n_frames, float *scores) {
   if (!h || !in || !scores) { set_error("jb200_dnn_score_host: null argument"); return JB200_ERR_ARG; }
+  h->layout_fixed = true;
+  const int T = n_frames - h->context + 1;
   if (T <= 0) return JB200_OK;
   JB_CUDA(cudaSetDevice(h->device));
   int rc = dnn_reserve(h, T); if (rc) return rc;
-  JB_CUDA(cudaMemcpyAsync(h->d_in, in, sizeof(float) * (size_t)T * h->in_dim, cudaMemcpyHostToDevice, h->stream));
-  rc = dnn_forward_device(h, h->d_in, T, h->d_rows, h->row_stride, h->stream); if (rc) return rc;
+  JB_CUDA(cudaMemcpyAsync(h->d_in, in, sizeof(float) * (size_t)n_frames * h->frame_len, cudaMemcpyHostToDevice, h->stream));
+  rc = dnn_forward_device(h, h->d_in, T, h->d_rows, h->row_stride, h->stream, SpliceMap()); if (rc) return rc;
   JB_CUDA(cudaMemcpy2DAsync(scores, sizeof(float) * h->out_dim, h->d_rows, sizeof(float) * h->row_stride, sizeof(float) * h->out_dim, T,
                             cudaMemcpyDeviceToHost, h->stream));
   JB_CUDA(cudaStreamSynchronize(h->stream));
