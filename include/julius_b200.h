@@ -230,6 +230,51 @@ int jb200_stream_status(jb200_decoder *d, int stream, int32_t *frames_done, int3
 int jb200_stream_partial(jb200_decoder *d, int stream, int32_t *words, int max_words, int32_t *n_words, float *score, int32_t *frame);
 int jb200_stream_result(jb200_decoder *d, int stream, const jb200_utt_result **utt, const jb200_atom **atoms, const int32_t **words);
 
+/* ------------------------------------------------------------------------------------
+ * Decoder groups: several recognition instances on one acoustic model score each input once.  Stands in for Julius'
+ * multi-decoding (-AM / -LM / -SR sections of a jconf), where every RecogProcess on one PROCESS_AM reads the same
+ * HMMWork and so the same outprob_cache (wchmm->hmmwrk = &am->hmmwrk, m_fusion.c:1182; decode_proceed runs every
+ * process on the frame, pass1.c:220-254).
+ * A group of 1..JB200_GROUP_MAX distinct decoders that all use the same jb200_gmm handle, and either all have the same
+ * jb200_dnn attached (attach it before creating the group) or none has one; trees (normal, multipath, grammar), beam
+ * widths, LMs and weights may differ.  Anything else is JB200_ERR_ARG, checked before the device is touched.  The group's
+ * capacity is the smallest max_utts and the smallest max_frames of its members.
+ * The group owns its feature and score-row buffers, the segment table and carry of a DNN that splices, and its own CUDA
+ * stream and events; the members' own buffers are not touched, so a member can still decode on its own between group
+ * calls.  A group call uploads and scores the input once, on the group's stream, and then launches the beam of every
+ * active member on that member's stream, reading the group's rows; an inactive member gets no launch and keeps its
+ * results.  Results are read from each member as usual: jb200_decoder_results (the host variants fetch every active
+ * member; after the device variant call jb200_decoder_fetch on it) and jb200_stream_status/_partial/_result.  A member's
+ * jb200_decoder_last_timing then shows its beam alone.
+ * Group batches are never sliced: jb200_decoder_set_pipeline does not apply to them, as it does not apply to score-row
+ * batches.  Destroy the group before any of its members.
+ * Decoders and groups that share one jb200_dnn may score on their own streams at any time: the handle orders its
+ * forwards on the device, each after the previous one (they share its activation buffers). 
+ * ---------------------------------------------------------------------------------- */
+#define JB200_GROUP_MAX 16
+typedef struct jb200_group jb200_group;
+int jb200_group_create(jb200_decoder *const *members, int n_members, jb200_group **out);
+void jb200_group_destroy(jb200_group *g);
+/* an inactive member (Julius -inactive, j_process_deactivate) is skipped by the group's calls until it is set active
+ * again; all are active after create.  While the group's stream is open the change is refused (JB200_ERR_ARG) as long
+ * as one of the member's streams is inside an utterance (started, not ended): a stream that missed feeds cannot go on. */
+int jb200_group_set_active(jb200_group *g, int member, int active);
+/* the batch entry points of a decoder (jb200_decode_batch_host/_device/_scores_host), for every active member at once */
+int jb200_group_decode_batch_host(jb200_group *g, const float *feats, const int32_t *frame_off, int n_utts);
+int jb200_group_decode_batch_device(jb200_group *g, const float *d_feats, const int32_t *frame_off, int n_utts);
+int jb200_group_decode_batch_scores_host(jb200_group *g, const float *scores, const int32_t *frame_off, int n_utts);
+/* Streams: every member opens n_streams streams (jb200_stream_open).  Until the group's next stream_open or batch, a
+ * member refuses its own jb200_stream_feed_* (JB200_ERR_ARG); a group feed scores the new frames once (a splicing DNN
+ * keeps its carry once, in the group) and advances every active member's streams as that member's own feed would.
+ * jb200_group_stream_restart restarts the stream of every active member; an inactive one keeps its last result. */
+int jb200_group_stream_open(jb200_group *g, int n_streams);
+int jb200_group_stream_restart(jb200_group *g, int stream);
+int jb200_group_stream_feed_host(jb200_group *g, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim);
+int jb200_group_stream_feed_scores_host(jb200_group *g, const float *scores, const int32_t *n_new, const uint8_t *last, int want_interim);
+/* timing of the last group call in milliseconds (CUDA events): [0] upload, [1] scoring, [2] beams (end of the scoring
+ * to the end of the last member's beam), [3] copy-back (0 after the device variant) */
+int jb200_group_last_timing(jb200_group *g, float ms[4]);
+
 #ifdef __cplusplus
 }
 #endif

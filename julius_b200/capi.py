@@ -87,6 +87,19 @@ def lib():
             L.jb200_stream_status.argtypes = [vp, C.c_int, D.I, D.I, D.I]
             L.jb200_stream_partial.argtypes = [vp, C.c_int, D.I, C.c_int, D.I, D.F, D.I]
             L.jb200_stream_result.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+        if hasattr(L, "jb200_group_create"):
+            U8 = C.POINTER(C.c_uint8)
+            L.jb200_group_create.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(vp)]
+            L.jb200_group_destroy.argtypes = [vp]
+            L.jb200_group_set_active.argtypes = [vp, C.c_int, C.c_int]
+            L.jb200_group_decode_batch_host.argtypes = [vp, D.F, D.I, C.c_int]
+            L.jb200_group_decode_batch_device.argtypes = [vp, vp, D.I, C.c_int]
+            L.jb200_group_decode_batch_scores_host.argtypes = [vp, D.F, D.I, C.c_int]
+            L.jb200_group_stream_open.argtypes = [vp, C.c_int]
+            L.jb200_group_stream_restart.argtypes = [vp, C.c_int]
+            L.jb200_group_stream_feed_host.argtypes = [vp, D.F, D.I, U8, C.c_int]
+            L.jb200_group_stream_feed_scores_host.argtypes = [vp, D.F, D.I, U8, C.c_int]
+            L.jb200_group_last_timing.argtypes = [vp, D.F]
         _lib = L
     return _lib
 
@@ -112,6 +125,32 @@ def _utt_result(u, pa: int, pw: int) -> dict:
     words = np.ctypeslib.as_array(C.cast(pw + int(u["word_offset"]) * 4, D.I), shape=(nw,)).copy().tolist() if nw > 0 else []
     return dict(status=int(u["status"]), n_frames=int(u["n_frames"]), atoms=atoms, words=words,
                 score=float(u["score"]), overflow=int(u["overflow"]))
+
+
+def _offsets(lengths):
+    off = np.zeros(len(lengths) + 1, np.int32)
+    np.cumsum(np.asarray(lengths, np.int64), out=off[1:])
+    return off
+
+
+def _batch(fn, h, arrays, what: str):
+    """one call of a host batch entry point on the concatenated arrays and their offsets"""
+    off = _offsets([len(x) for x in arrays])
+    cat = np.ascontiguousarray(np.concatenate(arrays, 0), np.float32)
+    _check(fn(h, _f(cat), off.ctypes.data_as(D.I), len(arrays)), what)
+
+
+def _feed(fn, h, n: int, chunks, last, interim: bool, what: str):
+    """one call of a stream feed entry point: the chunks packed stream-major, their counts and the end flags"""
+    dim = None
+    for c in chunks:
+        if c is not None and len(c):
+            dim = c.shape[1]
+    n_new = np.array([0 if c is None else len(c) for c in chunks], np.int32)
+    parts = [np.asarray(c, np.float32) for c in chunks if c is not None and len(c)]
+    cat = np.ascontiguousarray(np.concatenate(parts, 0)) if parts else np.zeros((1, dim or 1), np.float32)
+    lastv = np.zeros(n, np.uint8) if last is None else np.asarray(last, np.uint8)
+    _check(fn(h, _f(cat), n_new.ctypes.data_as(D.I), lastv.ctypes.data_as(C.POINTER(C.c_uint8)), 1 if interim else 0), what)
 
 
 class GmmScorer:
@@ -219,27 +258,15 @@ class Decoder:
         _check(lib().jb200_decoder_attach_dnn(self._h, dnn.handle), "jb200_decoder_attach_dnn")
         self.dnn = dnn
 
-    @staticmethod
-    def _offsets(lengths):
-        off = np.zeros(len(lengths) + 1, np.int32)
-        np.cumsum(np.asarray(lengths, np.int64), out=off[1:])
-        return off
-
     def decode(self, feats_list):
         """feats_list: list of [T_u, dim] arrays (host; front-end frames [N_u, frame_len] when the attached DNN splices).
         Returns list of result dicts."""
-        off = self._offsets([len(x) for x in feats_list])
-        cat = np.ascontiguousarray(np.concatenate(feats_list, 0), np.float32)
-        _check(lib().jb200_decode_batch_host(self._h, _f(cat), off.ctypes.data_as(D.I), len(feats_list)),
-               "jb200_decode_batch_host")
+        _batch(lib().jb200_decode_batch_host, self._h, feats_list, "jb200_decode_batch_host")
         self._last_n = len(feats_list)
         return self.results()
 
     def decode_scores(self, scores_list):
-        off = self._offsets([len(x) for x in scores_list])
-        cat = np.ascontiguousarray(np.concatenate(scores_list, 0), np.float32)
-        _check(lib().jb200_decode_batch_scores_host(self._h, _f(cat), off.ctypes.data_as(D.I), len(scores_list)),
-               "jb200_decode_batch_scores_host")
+        _batch(lib().jb200_decode_batch_scores_host, self._h, scores_list, "jb200_decode_batch_scores_host")
         self._last_n = len(scores_list)
         return self.results()
 
@@ -284,18 +311,8 @@ class Decoder:
 
     def stream_feed(self, chunks, last=None, interim: bool = False, scores: bool = False):
         """chunks: one [n_new, dim] array (or None / empty) per stream; last: per-stream end-of-utterance flags."""
-        n = self._st_n
-        dim = None
-        for c in chunks:
-            if c is not None and len(c):
-                dim = c.shape[1]
-        n_new = np.array([0 if c is None else len(c) for c in chunks], np.int32)
-        parts = [np.asarray(c, np.float32) for c in chunks if c is not None and len(c)]
-        cat = np.ascontiguousarray(np.concatenate(parts, 0)) if parts else np.zeros((1, dim or 1), np.float32)
-        lastv = np.zeros(n, np.uint8) if last is None else np.asarray(last, np.uint8)
         fn = lib().jb200_stream_feed_scores_host if scores else lib().jb200_stream_feed_host
-        _check(fn(self._h, _f(cat), n_new.ctypes.data_as(D.I), lastv.ctypes.data_as(C.POINTER(C.c_uint8)), 1 if interim else 0),
-               "jb200_stream_feed")
+        _feed(fn, self._h, self._st_n, chunks, last, interim, "jb200_stream_feed")
 
     def stream_status(self, stream: int) -> dict:
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
@@ -361,6 +378,80 @@ class Decoder:
     def close(self):
         if self._h:
             lib().jb200_decoder_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DecoderGroup:
+    """Recognition instances on one acoustic model (Julius multi-decoding): each batch or stream feed is scored once and
+    decoded by every active member.  Per-member results come from the members' own Decoder methods (results(),
+    stream_status(), stream_partial(), stream_result()).  Close the group before its members."""
+
+    def __init__(self, decoders):
+        self.members = list(decoders)
+        self._h = C.c_void_p()
+        hs = (C.c_void_p * max(len(self.members), 1))(*[d.handle_ptr() for d in self.members])
+        _check(lib().jb200_group_create(hs, len(self.members), C.byref(self._h)), "jb200_group_create")
+        self._active = [True] * len(self.members)
+        self._st_n = 0                  # until stream_open: the library refuses a feed
+
+    def set_active(self, member: int, active: bool):
+        _check(lib().jb200_group_set_active(self._h, member, 1 if active else 0), "jb200_group_set_active")
+        self._active[member] = bool(active)
+
+    def _results(self, n):
+        for d, a in zip(self.members, self._active):
+            if a:
+                d._last_n = n
+        return [d.results() if a else None for d, a in zip(self.members, self._active)]
+
+    def decode(self, feats_list):
+        """-> one list of result dicts per member (None for an inactive member)"""
+        _batch(lib().jb200_group_decode_batch_host, self._h, feats_list, "jb200_group_decode_batch_host")
+        return self._results(len(feats_list))
+
+    def decode_scores(self, scores_list):
+        _batch(lib().jb200_group_decode_batch_scores_host, self._h, scores_list, "jb200_group_decode_batch_scores_host")
+        return self._results(len(scores_list))
+
+    def decode_device(self, d_feats_ptr: int, frame_off: np.ndarray, fetch: bool = True):
+        frame_off = np.ascontiguousarray(frame_off, np.int32)
+        n = len(frame_off) - 1
+        _check(lib().jb200_group_decode_batch_device(self._h, d_feats_ptr, frame_off.ctypes.data_as(D.I), n),
+               "jb200_group_decode_batch_device")
+        for d, a in zip(self.members, self._active):
+            if a:
+                d._last_n = n
+                if fetch:
+                    _check(lib().jb200_decoder_fetch(d.handle_ptr()), "jb200_decoder_fetch")
+
+    def stream_open(self, n_streams: int = 1):
+        _check(lib().jb200_group_stream_open(self._h, n_streams), "jb200_group_stream_open")
+        self._st_n = n_streams
+        for d in self.members:
+            d._st_n = n_streams
+
+    def stream_restart(self, stream: int):
+        _check(lib().jb200_group_stream_restart(self._h, stream), "jb200_group_stream_restart")
+
+    def stream_feed(self, chunks, last=None, interim: bool = False, scores: bool = False):
+        """as Decoder.stream_feed, for every active member"""
+        fn = lib().jb200_group_stream_feed_scores_host if scores else lib().jb200_group_stream_feed_host
+        _feed(fn, self._h, self._st_n, chunks, last, interim, "jb200_group_stream_feed")
+
+    def timing(self):
+        ms = np.zeros(4, np.float32)
+        _check(lib().jb200_group_last_timing(self._h, _f(ms)), "jb200_group_last_timing")
+        return dict(h2d=float(ms[0]), score=float(ms[1]), beams=float(ms[2]), d2h=float(ms[3]))
+
+    def close(self):
+        if self._h:
+            lib().jb200_group_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

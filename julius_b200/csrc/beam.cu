@@ -2089,10 +2089,27 @@ __global__ void carry_update_kernel(const SpliceSeg *__restrict__ seg, const flo
 // =============================================================================================
 using namespace jb200;
 
-struct jb200_decoder {
+// What turns a batch's or a feed's input into score rows: the scorer, the feature and score-row buffers it fills, and for
+// a DNN that splices ctx input frames of fl floats into each network input (jb200_dnn_set_context) the segment table
+// (pinned staging copy and device copy, max_utts + 1 entries) and, per stream, the input frames of its utterance so far
+// and its last ctx - 1 of them on the device, in one of a pair of buffers (carry_cur) that a feed's update swaps.
+// A decoder has its own; a group (jb200_group_*) has one for all its members.
+struct RowSource {
   jb200_gmm *am = nullptr;
   jb200_dnn *dnn = nullptr;
-  int device = 0, dim = 0, S = 0;
+  int dim = 0, S = 0, row_stride = 0;
+  int max_utts = 0, max_frames = 0;
+  float *d_feats = nullptr, *d_rows = nullptr;
+  int ctx = 1, fl = 0;
+  SpliceSeg *h_splice = nullptr, *d_splice = nullptr;
+  float *d_carry[2] = {nullptr, nullptr}; int carry_cur = 0; size_t carry_floats = 0;
+  std::vector<int> st_in;
+  bool splices() const { return dnn && ctx > 1; }
+};
+
+struct jb200_decoder {
+  RowSource in;
+  int device = 0;
   int max_utts = 0, max_frames = 0;         // per batch: utterances, total frames
   int atoms_per_frame = 64;
   // the one home of every device pointer fixed at create; launch_beam sets only the chunk row, interim and atoms_in_place
@@ -2103,7 +2120,6 @@ struct jb200_decoder {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[5]{};
   // buffers the host writes and the kernel reads through P's const pointers
-  float *d_feats = nullptr, *d_rows = nullptr;
   int *d_frame_off = nullptr; long long *d_atom_off = nullptr;
   // host results (pinned)
   jb200_utt_result *h_results = nullptr; jb200_atom *h_atoms = nullptr; int *h_words = nullptr;
@@ -2131,13 +2147,8 @@ struct jb200_decoder {
   std::vector<int> st_t; std::vector<char> st_started, st_done;
   long long *h_aoff = nullptr;                  // pinned copy of the per-utterance atom offsets
   UttState *h_state = nullptr; int *h_interim_words = nullptr;
-  // a DNN that splices ctx input frames of fl floats into each network input (jb200_dnn_set_context): the segment table
-  // (pinned staging copy and device copy, max_utts + 1 entries), and per stream the input frames of its utterance so far
-  // and its last ctx - 1 of them on the device, in one of a pair of buffers (carry_cur) that a feed's update swaps
-  int ctx = 1, fl = 0;
-  SpliceSeg *h_splice = nullptr, *d_splice = nullptr;
-  float *d_carry[2] = {nullptr, nullptr}; int carry_cur = 0; size_t carry_floats = 0;
-  std::vector<int> st_in;
+  // the group whose open stream this decoder is in (jb200_group_stream_open): its own feeds are refused meanwhile
+  const jb200_group *stream_group = nullptr;
 };
 
 // from the shared-table arena when it has room, else an allocation of its own
@@ -2148,8 +2159,9 @@ static void *arena_take(jb200_decoder *d, size_t bytes) {
   d->arena_used += need;
   return p;
 }
-template <typename Tp>
-static int dev_alloc(jb200_decoder *d, size_t n, Tp **dst) {
+// Owner: a decoder or a group, which frees its dev_allocs and host_allocs when destroyed
+template <typename Owner, typename Tp>
+static int dev_alloc(Owner *d, size_t n, Tp **dst) {
   Tp *p = nullptr;
   JB_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(Tp)));
   d->dev_allocs.push_back(p);
@@ -2169,8 +2181,8 @@ static int dev_upload(jb200_decoder *d, const Tp *src, size_t n, const Tp **dst)
   *dst = p;
   return JB200_OK;
 }
-template <typename Tp>
-static int host_alloc(jb200_decoder *d, size_t n, Tp **dst) {
+template <typename Owner, typename Tp>
+static int host_alloc(Owner *d, size_t n, Tp **dst) {
   Tp *p = nullptr;
   JB_CUDA(cudaMallocHost(&p, n * sizeof(Tp)));
   d->host_allocs.push_back(p);
@@ -2360,7 +2372,7 @@ static int upload_lm(jb200_decoder *d, const jb200_tree_desc *t) {
   P.tail_silwid = t->tail_silwid; P.beam = t->beam_width;
   // cd sets come from the AM handle's descriptor: re-upload from the gmm handle is not exposed, so the
   // decoder asks the scorer for its device copies
-  gmm_cd_device(d->am, &P.cd_off, &P.cd_states, &P.iwcd_method, &P.iwcd_nbest);
+  gmm_cd_device(d->in.am, &P.cd_off, &P.cd_states, &P.iwcd_method, &P.iwcd_nbest);
   // inter-word bigram rows for every last word (the reference's iw_sc_cache, fully populated)
   const int *d_iso_word = nullptr;
   JB_RC(dev_upload(d, t->iso_word, (size_t)t->n_iso, &d_iso_word));
@@ -2448,8 +2460,8 @@ static int alloc_work(jb200_decoder *d, const jb200_tree_desc *t, const CutSizin
   JB_RC(dev_alloc(d, (size_t)mu * 8, &P.prof));
   JB_RC(dev_alloc(d, (size_t)mu + 1, &d->d_frame_off));
   JB_RC(dev_alloc(d, (size_t)mu + 1, &d->d_atom_off));
-  JB_RC(dev_alloc(d, (size_t)mf * d->dim, &d->d_feats));
-  JB_RC(dev_alloc(d, (size_t)mf * P.row_stride, &d->d_rows));
+  JB_RC(dev_alloc(d, (size_t)mf * d->in.dim, &d->in.d_feats));
+  JB_RC(dev_alloc(d, (size_t)mf * P.row_stride, &d->in.d_rows));
   JB_RC(host_alloc(d, (size_t)mu, &d->h_results));
   JB_RC(host_alloc(d, atoms_cap, &d->h_atoms));
   JB_RC(host_alloc(d, (size_t)mu * MAX_WORDS, &d->h_words));
@@ -2464,7 +2476,7 @@ static int alloc_work(jb200_decoder *d, const jb200_tree_desc *t, const CutSizin
   JB_RC(host_alloc(d, (size_t)mu + 1, &d->h_aoff));
   JB_RC(host_alloc(d, (size_t)mu, &d->h_state));
   JB_RC(host_alloc(d, (size_t)mu * MAX_WORDS, &d->h_interim_words));
-  P.rows = d->d_rows; P.frame_off = d->d_frame_off; P.atom_off = d->d_atom_off; P.chunk = d->d_chunk;
+  P.rows = d->in.d_rows; P.frame_off = d->d_frame_off; P.atom_off = d->d_atom_off; P.chunk = d->d_chunk;
   // the scoring stream of the batch pipeline gets the higher priority: its thread blocks take the room the token-passing
   // kernel leaves on every SM as soon as it is free
   int lo = 0, hi = 0;
@@ -2476,7 +2488,11 @@ static int alloc_work(jb200_decoder *d, const jb200_tree_desc *t, const CutSizin
   d->smem_bytes = cs.smem_bytes;
   d->beam = beam_kernel_for(t->lm_type == JB200_LM_DFA, P.multipath, check_heap);
   const void *kern = (const void *)d->beam;
-  JB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
+  // the limit belongs to the kernel, which decoders of other beam widths share: only ever raise it
+  cudaFuncAttributes fa;
+  JB_CUDA(cudaFuncGetAttributes(&fa, kern));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < d->smem_bytes)
+    JB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->smem_bytes));
   int per_sm = 0, sms = 0;
   JB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BEAM_THREADS, d->smem_bytes));
   JB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d->device));
@@ -2487,9 +2503,9 @@ static int alloc_work(jb200_decoder *d, const jb200_tree_desc *t, const CutSizin
 
 // the device half of jb200_decoder_create, on a checked tree
 static int build_decoder(jb200_decoder *d, const jb200_tree_desc *t, jb200_gmm *am, int max_utts, int max_frames) {
-  d->am = am; d->device = gmm_device(am); d->dim = gmm_dim(am); d->S = jb200_gmm_n_states(am);
-  d->P.row_stride = (d->S + 3) & ~3;
-  d->max_utts = max_utts; d->max_frames = max_frames;
+  d->in.am = am; d->device = gmm_device(am); d->in.dim = gmm_dim(am); d->in.S = jb200_gmm_n_states(am);
+  d->in.row_stride = d->P.row_stride = (d->in.S + 3) & ~3;
+  d->max_utts = d->in.max_utts = max_utts; d->max_frames = d->in.max_frames = max_frames;
   if (const char *e = getenv("JB200_ATOMS_PER_FRAME")) d->atoms_per_frame = std::max(4, atoi(e));
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
@@ -2543,7 +2559,7 @@ static int layout_utts(jb200_decoder *d, const int32_t *frame_off, int n_utts) {
 static void plan_slices(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
   int maxT = 0;
   for (int u = 0; u < n_utts; u++) maxT = std::max(maxT, frame_off[u + 1] - frame_off[u]);
-  int F = (allow_pipe && !d->dnn && d->pipe_frames > 0) ? d->pipe_frames : 0;
+  int F = (allow_pipe && !d->in.dnn && d->pipe_frames > 0) ? d->pipe_frames : 0;
   int nch = 1;
   if (F > 0) {
     nch = (maxT + F - 1) / F;
@@ -2576,16 +2592,24 @@ static void plan_slices(jb200_decoder *d, const int32_t *frame_off, int n_utts, 
   }
 }
 
-static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
-  if (!d || !frame_off || n_utts < 1) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
-  if (n_utts > d->max_utts) { set_error("batch of %d utterances exceeds decoder capacity %d", n_utts, d->max_utts); return JB200_ERR_CAPACITY; }
+// a batch of n_utts utterances whose decoded frames start at frame_off fits the capacity of s
+static int check_batch(const RowSource &s, const int32_t *frame_off, int n_utts) {
+  if (!frame_off || n_utts < 1) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
+  if (n_utts > s.max_utts) { set_error("batch of %d utterances exceeds decoder capacity %d", n_utts, s.max_utts); return JB200_ERR_CAPACITY; }
   const int total = frame_off[n_utts] - frame_off[0];
   if (frame_off[0] != 0) { set_error("frame_off[0] must be 0"); return JB200_ERR_ARG; }
-  if (total > d->max_frames) { set_error("batch of %d frames exceeds decoder capacity %d", total, d->max_frames); return JB200_ERR_CAPACITY; }
+  if (total > s.max_frames) { set_error("batch of %d frames exceeds decoder capacity %d", total, s.max_frames); return JB200_ERR_CAPACITY; }
+  return JB200_OK;
+}
+
+static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts, bool allow_pipe) {
+  if (!d) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
+  JB_RC(check_batch(d->in, frame_off, n_utts));
+  const int total = frame_off[n_utts];
   JB_CUDA(cudaSetDevice(d->device));
   JB_CUDA(cudaStreamSynchronize(d->stream));   // the staging buffers below may still feed the previous batch's copies
   JB_RC(layout_utts(d, frame_off, n_utts));
-  d->stream_mode = false;
+  d->stream_mode = false; d->stream_group = nullptr;
   plan_slices(d, frame_off, n_utts, allow_pipe);
   const int mu = d->max_utts;
   JB_CUDA(cudaMemcpyAsync(d->d_chunk, d->h_chunk, sizeof(ChunkDesc) * (size_t)d->n_chunks * mu, cudaMemcpyHostToDevice, d->stream));
@@ -2597,8 +2621,10 @@ static int prepare_batch(jb200_decoder *d, const int32_t *frame_off, int n_utts,
   return JB200_OK;
 }
 
-static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index, int interim = 0) {
+// the beam kernel over chunk chunk_index of n_utts utterances; rows: a group's score rows instead of the decoder's own
+static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index, int interim = 0, const float *rows = nullptr) {
   BeamParams P = d->P;
+  if (rows) P.rows = rows;
   P.chunk = d->d_chunk + (size_t)chunk_index * d->max_utts;
   P.interim = interim; P.atoms_in_place = d->stream_mode ? 1 : 0;
   d->beam<<<n_utts, BEAM_THREADS, d->smem_bytes, d->stream>>>(P);
@@ -2606,11 +2632,11 @@ static int launch_beam(jb200_decoder *d, int n_utts, int chunk_index, int interi
   return JB200_OK;
 }
 
-// scores T frames of device features into the score rows, on the main stream; a splicing DNN reads its input rows
+// scores T frames of device features into the source's score rows, on stream st; a splicing DNN reads its input rows
 // through sm
-static int score_frames(jb200_decoder *d, const float *d_feats, int T, const SpliceMap &sm = SpliceMap()) {
-  return d->dnn ? dnn_forward_device(d->dnn, d_feats, T, d->d_rows, d->P.row_stride, d->stream, sm)
-                : gmm_launch_states(d->am, d_feats, T, d->d_rows, d->P.row_stride, d->stream, nullptr, nullptr, 0);
+static int score_frames(RowSource &s, cudaStream_t st, const float *d_feats, int T, const SpliceMap &sm = SpliceMap()) {
+  return s.dnn ? dnn_forward_device(s.dnn, d_feats, T, s.d_rows, s.row_stride, st, sm)
+               : gmm_launch_states(s.am, d_feats, T, s.d_rows, s.row_stride, st, nullptr, nullptr, 0);
 }
 
 // scoring of a prepared batch's features at d_feats, time slice by time slice on the scoring stream, beside the token
@@ -2623,7 +2649,7 @@ static int run_pipeline(jb200_decoder *d, const float *d_feats, int n_utts) {
   JB_CUDA(cudaEventRecord(d->ev_score_begin, d->score_stream));
   for (int c = 0; c < d->n_chunks; c++) {
     const int *ds = d->d_seg + (size_t)c * segw;
-    JB_RC(gmm_launch_states(d->am, d_feats, d->slice_frames[c], d->d_rows, d->P.row_stride, d->score_stream, ds, ds + mu + 1, d->slice_nseg[c]));
+    JB_RC(gmm_launch_states(d->in.am, d_feats, d->slice_frames[c], d->in.d_rows, d->P.row_stride, d->score_stream, ds, ds + mu + 1, d->slice_nseg[c]));
     JB_CUDA(cudaEventRecord(d->ev_slice[c], d->score_stream));
   }
   JB_CUDA(cudaEventRecord(d->ev_score_end, d->score_stream));
@@ -2681,31 +2707,40 @@ extern "C" int jb200_decoder_phase_cycles(jb200_decoder *d, int64_t *cycles, int
   return JB200_OK;
 }
 
+// a row source's splice set-up for input frames fl wide, ctx to a network input: with ctx > 1 the segment table and the
+// carry of max_utts streams
+template <typename Owner>
+static int reserve_splice(Owner *o, RowSource &s, int ctx, int fl) {
+  if (ctx > 1) {
+    if (!s.d_splice) {
+      JB_RC(dev_alloc(o, (size_t)s.max_utts + 1, &s.d_splice));
+      JB_RC(host_alloc(o, (size_t)s.max_utts + 1, &s.h_splice));
+    }
+    const size_t carry = (size_t)s.max_utts * (ctx - 1) * fl;
+    if (carry > s.carry_floats) {
+      for (auto &c : s.d_carry) JB_RC(dev_alloc(o, carry, &c));
+      s.carry_floats = carry;
+    }
+  }
+  s.ctx = ctx; s.fl = fl;
+  return JB200_OK;
+}
+
 extern "C" int jb200_decoder_attach_dnn(jb200_decoder *d, jb200_dnn *dnn) {
   if (!d || !dnn) { set_error("null argument"); return JB200_ERR_ARG; }
-  if (jb200_dnn_out_dim(dnn) != d->S) { set_error("DNN has %d outputs but the HMM set has %d states", jb200_dnn_out_dim(dnn), d->S); return JB200_ERR_ARG; }
+  if (jb200_dnn_out_dim(dnn) != d->in.S) { set_error("DNN has %d outputs but the HMM set has %d states", jb200_dnn_out_dim(dnn), d->in.S); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(d->device));
   const int dim = jb200_dnn_in_dim(dnn);
-  if (dim != d->dim) {
+  if (dim != d->in.dim) {
     // the feature buffer was sized for the AM's dimension; re-size it for the DNN's input width
     float *nf = nullptr;
     JB_RC(dev_alloc(d, (size_t)d->max_frames * dim, &nf));
-    d->d_feats = nf; d->dim = dim;
+    d->in.d_feats = nf; d->in.dim = dim;
   }
   // input frames of a splicing DNN are dim / ctx wide: max_frames network inputs' worth of them fit in d_feats as it is
-  const int ctx = dnn_fix_context(dnn), fl = dim / ctx;
-  if (ctx > 1) {
-    if (!d->d_splice) {
-      JB_RC(dev_alloc(d, (size_t)d->max_utts + 1, &d->d_splice));
-      JB_RC(host_alloc(d, (size_t)d->max_utts + 1, &d->h_splice));
-    }
-    const size_t carry = (size_t)d->max_utts * (ctx - 1) * fl;
-    if (carry > d->carry_floats) {
-      for (auto &c : d->d_carry) JB_RC(dev_alloc(d, carry, &c));
-      d->carry_floats = carry;
-    }
-  }
-  d->dnn = dnn; d->ctx = ctx; d->fl = fl;
+  const int ctx = dnn_fix_context(dnn);
+  JB_RC(reserve_splice(d, d->in, ctx, dim / ctx));
+  d->in.dnn = dnn;
   return JB200_OK;
 }
 
@@ -2753,52 +2788,78 @@ enum BatchInput { FEATS_DEVICE, FEATS_HOST, SCORES_HOST };
 // A batch for a splicing DNN: frame_off counts input frames, and utterance u of N_u of them decodes
 // max(0, N_u - ctx + 1) frames (an input shorter than the window decodes none, Julius' "input too short",
 // wav2mfcc.c:132-135).  rows_off gets the offsets of the decoded frames.
-static int splice_rows(jb200_decoder *d, bool host_feats, const int32_t *frame_off, int n_utts, std::vector<int32_t> &rows_off) {
+static int splice_rows(const RowSource &s, bool host_feats, const int32_t *frame_off, int n_utts, std::vector<int32_t> &rows_off) {
   if (!frame_off || n_utts < 1) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
   if (frame_off[0] != 0) { set_error("frame_off[0] must be 0"); return JB200_ERR_ARG; }
   rows_off.assign(n_utts + 1, 0);
   for (int u = 0; u < n_utts; u++) {
     const int N = frame_off[u + 1] - frame_off[u];
     if (N < 0) { set_error("utterance %d has %d input frames", u, N); return JB200_ERR_ARG; }
-    rows_off[u + 1] = rows_off[u] + std::max(0, N - d->ctx + 1);
+    rows_off[u + 1] = rows_off[u] + std::max(0, N - s.ctx + 1);
   }
-  if (host_feats && (long long)frame_off[n_utts] * d->fl > (long long)d->max_frames * d->dim) {
-    set_error("batch of %d input frames exceeds decoder capacity %d", frame_off[n_utts], d->max_frames * d->ctx);
+  if (host_feats && (long long)frame_off[n_utts] * s.fl > (long long)s.max_frames * s.dim) {
+    set_error("batch of %d input frames exceeds decoder capacity %d", frame_off[n_utts], s.max_frames * s.ctx);
     return JB200_ERR_CAPACITY;
   }
+  return JB200_OK;
+}
+
+// Getting a batch's rows, step 1, on the host: *rows gets the offsets of the decoded frames, which are frame_off unless
+// a splicing DNN takes features (then they are kept in rows_off).
+static int batch_rows_off(const RowSource &s, BatchInput in, const float *x, const int32_t *frame_off, int n_utts,
+                          std::vector<int32_t> &rows_off, const int32_t **rows) {
+  if (in != FEATS_DEVICE && !x) { set_error(in == SCORES_HOST ? "null scores" : "null feats"); return JB200_ERR_ARG; }
+  *rows = frame_off;
+  if (in != SCORES_HOST && s.splices()) {
+    JB_RC(splice_rows(s, in == FEATS_HOST, frame_off, n_utts, rows_off));
+    *rows = rows_off.data();
+  }
+  return JB200_OK;
+}
+
+// Getting a batch's rows, step 2, on stream st once the batch is laid out: uploads what the call hands in, records ev_in,
+// and with score scores the features into s.d_rows.  *d_x gets the features on the device (for the batch pipeline, which
+// scores them itself).  The staging segment table must be free: st has no copy from it pending.
+static int batch_rows(RowSource &s, cudaStream_t st, BatchInput in, const float *x, const int32_t *frame_off, const int32_t *rows,
+                      int n_utts, cudaEvent_t ev_in, bool score, const float **d_x) {
+  const bool splice = in != SCORES_HOST && s.splices();
+  const int total = rows[n_utts];
+  SpliceMap sm;
+  if (splice) {
+    // utterance u's decoded frames read the windows of its own input frames
+    for (int u = 0; u <= n_utts; u++)
+      s.h_splice[u] = SpliceSeg{rows[u], frame_off[u], 0, 0, u < n_utts ? frame_off[u + 1] - frame_off[u] : 0};
+    JB_CUDA(cudaMemcpyAsync(s.d_splice, s.h_splice, sizeof(SpliceSeg) * (n_utts + 1), cudaMemcpyHostToDevice, st));
+    sm.seg = s.d_splice; sm.nseg = n_utts;
+  }
+  if (in == FEATS_HOST) {
+    const size_t n = splice ? (size_t)frame_off[n_utts] * s.fl : (size_t)total * s.dim;
+    JB_CUDA(cudaMemcpyAsync(s.d_feats, x, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    x = s.d_feats;
+  }
+  if (in == SCORES_HOST)
+    JB_CUDA(cudaMemcpy2DAsync(s.d_rows, sizeof(float) * s.row_stride, x, sizeof(float) * s.S, sizeof(float) * s.S, total,
+                              cudaMemcpyHostToDevice, st));
+  JB_CUDA(cudaEventRecord(ev_in, st));
+  *d_x = x;
+  if (score && in != SCORES_HOST) JB_RC(score_frames(s, st, x, total, sm));
   return JB200_OK;
 }
 
 // One batch, ev[0..3] around the upload, the scoring and the beam.  The host variants fetch the results; for device
 // features that is left to jb200_decoder_fetch.  Score rows are never pipelined.
 static int decode_batch(jb200_decoder *d, BatchInput in, const float *x, const int32_t *frame_off, int n_utts) {
-  if (in != FEATS_DEVICE && !x) { set_error(in == SCORES_HOST ? "null scores" : "null feats"); return JB200_ERR_ARG; }
-  const bool splice = in != SCORES_HOST && d && d->dnn && d->ctx > 1;
+  if (!d) { set_error("decode: bad argument"); return JB200_ERR_ARG; }
   std::vector<int32_t> rows_off;
-  if (splice) JB_RC(splice_rows(d, in == FEATS_HOST, frame_off, n_utts, rows_off));
-  JB_RC(prepare_batch(d, splice ? rows_off.data() : frame_off, n_utts, in != SCORES_HOST));
+  const int32_t *rows = nullptr;
+  JB_RC(batch_rows_off(d->in, in, x, frame_off, n_utts, rows_off, &rows));
+  JB_RC(prepare_batch(d, rows, n_utts, in != SCORES_HOST));
   JB_CUDA(cudaEventRecord(d->ev[0], d->stream));
-  SpliceMap sm;
-  if (splice) {
-    // utterance u's decoded frames read the windows of its own input frames
-    for (int u = 0; u <= n_utts; u++)
-      d->h_splice[u] = SpliceSeg{rows_off[u], frame_off[u], 0, 0, u < n_utts ? frame_off[u + 1] - frame_off[u] : 0};
-    JB_CUDA(cudaMemcpyAsync(d->d_splice, d->h_splice, sizeof(SpliceSeg) * (n_utts + 1), cudaMemcpyHostToDevice, d->stream));
-    sm.seg = d->d_splice; sm.nseg = n_utts;
-  }
-  if (in == FEATS_HOST) {
-    const size_t n = splice ? (size_t)frame_off[n_utts] * d->fl : (size_t)d->last_total_frames * d->dim;
-    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * n, cudaMemcpyHostToDevice, d->stream));
-    x = d->d_feats;
-  }
-  if (in == SCORES_HOST)
-    JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->P.row_stride, x, sizeof(float) * d->S, sizeof(float) * d->S,
-                              d->last_total_frames, cudaMemcpyHostToDevice, d->stream));
-  JB_CUDA(cudaEventRecord(d->ev[1], d->stream));
+  const float *d_x = nullptr;
+  JB_RC(batch_rows(d->in, d->stream, in, x, frame_off, rows, n_utts, d->ev[1], !d->last_piped, &d_x));
   if (d->last_piped) {
-    JB_RC(run_pipeline(d, x, n_utts));
+    JB_RC(run_pipeline(d, d_x, n_utts));
   } else {
-    if (in != SCORES_HOST) JB_RC(score_frames(d, x, d->last_total_frames, sm));
     JB_CUDA(cudaEventRecord(d->ev[2], d->stream));
     JB_RC(launch_beam(d, n_utts, 0));
   }
@@ -2830,8 +2891,8 @@ extern "C" int jb200_stream_open(jb200_decoder *d, int n_streams) {
     for (int u = 0; u < d->st_n; u++) if (d->st_started[u] && !d->st_done[u]) JB_RC(reset_slots(d, u, 1));
   const int cap = std::min(d->max_frames / n_streams, 32767);
   if (cap < 1) { set_error("decoder capacity of %d frames is too small for %d streams", d->max_frames, n_streams); return JB200_ERR_CAPACITY; }
-  d->stream_mode = true; d->st_n = n_streams; d->st_cap = cap;
-  d->st_t.assign(n_streams, 0); d->st_started.assign(n_streams, 0); d->st_done.assign(n_streams, 0); d->st_in.assign(n_streams, 0);
+  d->stream_mode = true; d->stream_group = nullptr; d->st_n = n_streams; d->st_cap = cap;
+  d->st_t.assign(n_streams, 0); d->st_started.assign(n_streams, 0); d->st_done.assign(n_streams, 0); d->in.st_in.assign(n_streams, 0);
   std::vector<int32_t> frame_off(n_streams + 1);
   for (int u = 0; u <= n_streams; u++) frame_off[u] = u * cap;
   JB_RC(layout_utts(d, frame_off.data(), n_streams));
@@ -2840,26 +2901,29 @@ extern "C" int jb200_stream_open(jb200_decoder *d, int n_streams) {
   return JB200_OK;
 }
 
-// device part of a feed: rows of the n_new[s] new decoded frames are in d_rows, packed stream-major
-static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t *last, int want_interim) {
+// Advancing the beams of a feed, step 1: the beam launch over the rows of the rows[s] new decoded frames of every stream,
+// packed stream-major (rows: a group's score rows instead of the decoder's own), and the copies of what the feed
+// returns.  *launched = false when no stream had anything to do.
+static int stream_launch(jb200_decoder *d, const int32_t *rows, const uint8_t *last, int want_interim, const float *d_rows, bool *launched) {
   int pack = 0;
   bool any = false, fin_any = false;
   for (int u = 0; u < d->st_n; u++) {
-    ChunkDesc k; k.t0 = d->st_t[u]; k.t1 = k.t0 + n_new[u]; k.row_base = pack - k.t0; k.flags = 0;
+    ChunkDesc k; k.t0 = d->st_t[u]; k.t1 = k.t0 + rows[u]; k.row_base = pack - k.t0; k.flags = 0;
     const bool fin = last && last[u];
-    if (d->st_done[u] || (n_new[u] == 0 && !fin)) k.flags = CHUNK_SKIP;
+    if (d->st_done[u] || (rows[u] == 0 && !fin)) k.flags = CHUNK_SKIP;
     else {
       if (!d->st_started[u]) k.flags |= CHUNK_FIRST;
       if (fin) k.flags |= CHUNK_FINAL;
       any = true; fin_any |= fin;
     }
     d->h_chunk[u] = k;
-    pack += n_new[u];
+    pack += rows[u];
   }
+  *launched = any;
   if (!any) return JB200_OK;
   const BeamParams &P = d->P;
   JB_CUDA(cudaMemcpyAsync(d->d_chunk, d->h_chunk, sizeof(ChunkDesc) * (size_t)d->st_n, cudaMemcpyHostToDevice, d->stream));
-  JB_RC(launch_beam(d, d->st_n, 0, want_interim));
+  JB_RC(launch_beam(d, d->st_n, 0, want_interim, d_rows));
   // results of the streams that ended; interim state of the others
   if (fin_any) {
     JB_CUDA(cudaMemcpyAsync(d->h_results, P.results, sizeof(jb200_utt_result) * d->st_n, cudaMemcpyDeviceToHost, d->stream));
@@ -2868,6 +2932,13 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
   JB_CUDA(cudaMemcpyAsync(d->h_state, P.state, sizeof(UttState) * (size_t)d->st_n, cudaMemcpyDeviceToHost, d->stream));
   if (want_interim)
     JB_CUDA(cudaMemcpyAsync(d->h_interim_words, P.interim_words, sizeof(int) * (size_t)d->st_n * MAX_WORDS, cudaMemcpyDeviceToHost, d->stream));
+  return JB200_OK;
+}
+
+// Advancing the beams of a feed, step 2, after a launch: waits for it, moves the streams on and fetches the atoms of the
+// streams that ended
+static int stream_collect(jb200_decoder *d) {
+  const BeamParams &P = d->P;
   JB_CUDA(cudaStreamSynchronize(d->stream));
   d->last_d2h = 0;
   for (int u = 0; u < d->st_n; u++) {
@@ -2885,58 +2956,98 @@ static int stream_advance(jb200_decoder *d, const int32_t *n_new, const uint8_t 
   return JB200_OK;
 }
 
-// jb200_stream_feed_host / _scores_host: the new frames of every stream, packed stream-major, as features or as score rows.
-// For a splicing DNN the features are input frames: stream s's window is the last min(ctx - 1, have) frames it was fed
-// before (have = its input frames so far) followed by its n_new[s] new ones, which give
-// max(0, have + n_new[s] - ctx + 1) - max(0, have - ctx + 1) decoded frames (splice_mfcc: nothing until ctx frames have
-// arrived, then one per frame).
-static int stream_feed(jb200_decoder *d, bool scores, const float *x, const int32_t *n_new, const uint8_t *last, int want_interim) {
-  if (!d || !n_new) { set_error("jb200_stream_feed: bad argument"); return JB200_ERR_ARG; }
-  if (!d->stream_mode) { set_error("jb200_stream_feed: call jb200_stream_open first"); return JB200_ERR_ARG; }
-  const bool splice = !scores && d->dnn && d->ctx > 1;
-  std::vector<int32_t> rows(d->st_n);           // decoded frames of each stream in this feed
-  int tot = 0, tot_rows = 0;
-  for (int u = 0; u < d->st_n; u++) {
+// Getting a feed's rows, step 1: rows[s], the frames stream s decodes from its n_new[s] new ones.  For a splicing DNN the
+// features are input frames: stream s's window is the last min(ctx - 1, have) frames it was fed before (have = its input
+// frames so far) followed by its n_new[s] new ones, which give max(0, have + n_new[s] - ctx + 1) - max(0, have - ctx + 1)
+// decoded frames (splice_mfcc: nothing until ctx frames have arrived, then one per frame).
+static int feed_rows(const RowSource &s, bool scores, const int32_t *n_new, int n, std::vector<int32_t> &rows) {
+  const bool splice = !scores && s.splices();
+  rows.assign(n, 0);
+  for (int u = 0; u < n; u++) {
     if (n_new[u] < 0) { set_error("stream %d: negative frame count", u); return JB200_ERR_ARG; }
-    if (d->st_done[u] && n_new[u] > 0) { set_error("stream %d has ended; restart it before feeding more frames", u); return JB200_ERR_ARG; }
-    rows[u] = splice ? std::max(0, d->st_in[u] + n_new[u] - d->ctx + 1) - std::max(0, d->st_in[u] - d->ctx + 1) : n_new[u];
-    if (d->st_t[u] + rows[u] > d->st_cap) { set_error("stream %d: %d frames exceed the per-stream capacity %d", u, d->st_t[u] + rows[u], d->st_cap); return JB200_ERR_CAPACITY; }
-    tot += n_new[u]; tot_rows += rows[u];
+    rows[u] = splice ? std::max(0, s.st_in[u] + n_new[u] - s.ctx + 1) - std::max(0, s.st_in[u] - s.ctx + 1) : n_new[u];
   }
-  if (tot_rows > d->max_frames) { set_error("%d new frames exceed decoder capacity %d", tot_rows, d->max_frames); return JB200_ERR_CAPACITY; }
-  if (splice && (long long)tot * d->fl > (long long)d->max_frames * d->dim) {
-    set_error("%d new input frames exceed decoder capacity %d", tot, d->max_frames * d->ctx);
+  return JB200_OK;
+}
+
+// a decoder's streams can take rows[s] more frames each: none has ended, none goes past the per-stream capacity
+static int check_feed(const jb200_decoder *d, const int32_t *n_new, const int32_t *rows) {
+  for (int u = 0; u < d->st_n; u++) {
+    if (d->st_done[u] && n_new[u] > 0) { set_error("stream %d has ended; restart it before feeding more frames", u); return JB200_ERR_ARG; }
+    if (d->st_t[u] + rows[u] > d->st_cap) { set_error("stream %d: %d frames exceed the per-stream capacity %d", u, d->st_t[u] + rows[u], d->st_cap); return JB200_ERR_CAPACITY; }
+  }
+  return JB200_OK;
+}
+
+// Getting a feed's rows, step 2: the feed fits the buffers of s
+static int feed_totals(const RowSource &s, bool scores, const float *x, const int32_t *n_new, const int32_t *rows, int n) {
+  long long tot = 0, tot_rows = 0;
+  for (int u = 0; u < n; u++) { tot += n_new[u]; tot_rows += rows[u]; }
+  if (tot_rows > s.max_frames) { set_error("%lld new frames exceed decoder capacity %d", tot_rows, s.max_frames); return JB200_ERR_CAPACITY; }
+  if (!scores && s.splices() && tot * s.fl > (long long)s.max_frames * s.dim) {
+    set_error("%lld new input frames exceed decoder capacity %d", tot, s.max_frames * s.ctx);
     return JB200_ERR_CAPACITY;
   }
   if (tot > 0 && !x) { set_error(scores ? "null scores" : "null feats"); return JB200_ERR_ARG; }
-  JB_CUDA(cudaSetDevice(d->device));
-  if (tot > 0 && scores)
-    JB_CUDA(cudaMemcpy2DAsync(d->d_rows, sizeof(float) * d->P.row_stride, x, sizeof(float) * d->S, sizeof(float) * d->S, tot, cudaMemcpyHostToDevice, d->stream));
-  else if (tot > 0 && !splice) {
-    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)tot * d->dim, cudaMemcpyHostToDevice, d->stream));
-    JB_RC(score_frames(d, d->d_feats, tot));
-  } else if (tot > 0) {
-    JB_CUDA(cudaStreamSynchronize(d->stream));   // the staging segment table may still feed the last feed's copy
+  return JB200_OK;
+}
+
+// Getting a feed's rows, step 3, on stream st: uploads the new frames of every stream, packed stream-major, as features or
+// as score rows, and scores the features into s.d_rows; a splicing DNN's streams move their carry on.
+// ev_in (may be null) is recorded once the input is on the device.
+static int feed_score(RowSource &s, cudaStream_t st, bool scores, const float *x, const int32_t *n_new, const int32_t *rows, int n,
+                      cudaEvent_t ev_in) {
+  int tot = 0, tot_rows = 0;
+  for (int u = 0; u < n; u++) { tot += n_new[u]; tot_rows += rows[u]; }
+  if (tot == 0) {
+    if (ev_in) JB_CUDA(cudaEventRecord(ev_in, st));
+    return JB200_OK;
+  }
+  if (scores) {
+    JB_CUDA(cudaMemcpy2DAsync(s.d_rows, sizeof(float) * s.row_stride, x, sizeof(float) * s.S, sizeof(float) * s.S, tot, cudaMemcpyHostToDevice, st));
+    if (ev_in) JB_CUDA(cudaEventRecord(ev_in, st));
+  } else if (!s.splices()) {
+    JB_CUDA(cudaMemcpyAsync(s.d_feats, x, sizeof(float) * (size_t)tot * s.dim, cudaMemcpyHostToDevice, st));
+    if (ev_in) JB_CUDA(cudaEventRecord(ev_in, st));
+    JB_RC(score_frames(s, st, s.d_feats, tot));
+  } else {
+    JB_CUDA(cudaStreamSynchronize(st));   // the staging segment table may still feed the last feed's copy
     int pack_in = 0, pack_rows = 0;
-    for (int u = 0; u < d->st_n; u++) {
-      const int have = std::min(d->ctx - 1, d->st_in[u]);
-      d->h_splice[u] = SpliceSeg{pack_rows, pack_in, u * (d->ctx - 1), have, have + n_new[u]};
+    for (int u = 0; u < n; u++) {
+      const int have = std::min(s.ctx - 1, s.st_in[u]);
+      s.h_splice[u] = SpliceSeg{pack_rows, pack_in, u * (s.ctx - 1), have, have + n_new[u]};
       pack_in += n_new[u]; pack_rows += rows[u];
     }
-    d->h_splice[d->st_n] = SpliceSeg{pack_rows, pack_in, 0, 0, 0};
-    JB_CUDA(cudaMemcpyAsync(d->d_splice, d->h_splice, sizeof(SpliceSeg) * (d->st_n + 1), cudaMemcpyHostToDevice, d->stream));
-    JB_CUDA(cudaMemcpyAsync(d->d_feats, x, sizeof(float) * (size_t)tot * d->fl, cudaMemcpyHostToDevice, d->stream));
+    s.h_splice[n] = SpliceSeg{pack_rows, pack_in, 0, 0, 0};
+    JB_CUDA(cudaMemcpyAsync(s.d_splice, s.h_splice, sizeof(SpliceSeg) * (n + 1), cudaMemcpyHostToDevice, st));
+    JB_CUDA(cudaMemcpyAsync(s.d_feats, x, sizeof(float) * (size_t)tot * s.fl, cudaMemcpyHostToDevice, st));
+    if (ev_in) JB_CUDA(cudaEventRecord(ev_in, st));
     SpliceMap sm;
-    sm.seg = d->d_splice; sm.nseg = d->st_n; sm.carry = d->d_carry[d->carry_cur];
-    JB_RC(score_frames(d, d->d_feats, tot_rows, sm));
+    sm.seg = s.d_splice; sm.nseg = n; sm.carry = s.d_carry[s.carry_cur];
+    JB_RC(score_frames(s, st, s.d_feats, tot_rows, sm));
     // after the scoring has read the carry, in stream order: the new carry goes to the other buffer
-    carry_update_kernel<<<d->st_n, 128, 0, d->stream>>>(d->d_splice, d->d_feats, d->d_carry[d->carry_cur], d->d_carry[d->carry_cur ^ 1],
-                                                        d->ctx - 1, d->fl);
+    carry_update_kernel<<<n, 128, 0, st>>>(s.d_splice, s.d_feats, s.d_carry[s.carry_cur], s.d_carry[s.carry_cur ^ 1], s.ctx - 1, s.fl);
     JB_LAUNCH_CHECK();
-    d->carry_cur ^= 1;
-    for (int u = 0; u < d->st_n; u++) d->st_in[u] += n_new[u];
+    s.carry_cur ^= 1;
+    for (int u = 0; u < n; u++) s.st_in[u] += n_new[u];
   }
-  return stream_advance(d, rows.data(), last, want_interim);
+  return JB200_OK;
+}
+
+// jb200_stream_feed_host / _scores_host: the new frames of every stream, packed stream-major, as features or as score rows
+static int stream_feed(jb200_decoder *d, bool scores, const float *x, const int32_t *n_new, const uint8_t *last, int want_interim) {
+  if (!d || !n_new) { set_error("jb200_stream_feed: bad argument"); return JB200_ERR_ARG; }
+  if (!d->stream_mode) { set_error("jb200_stream_feed: call jb200_stream_open first"); return JB200_ERR_ARG; }
+  if (d->stream_group) { set_error("jb200_stream_feed: the decoder is in an open group stream; feed the group"); return JB200_ERR_ARG; }
+  std::vector<int32_t> rows;                    // decoded frames of each stream in this feed
+  JB_RC(feed_rows(d->in, scores, n_new, d->st_n, rows));
+  JB_RC(check_feed(d, n_new, rows.data()));
+  JB_RC(feed_totals(d->in, scores, x, n_new, rows.data(), d->st_n));
+  JB_CUDA(cudaSetDevice(d->device));
+  JB_RC(feed_score(d->in, d->stream, scores, x, n_new, rows.data(), d->st_n, nullptr));
+  bool launched = false;
+  JB_RC(stream_launch(d, rows.data(), last, want_interim, nullptr, &launched));
+  return launched ? stream_collect(d) : JB200_OK;
 }
 
 extern "C" int jb200_stream_feed_host(jb200_decoder *d, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim) {
@@ -2954,7 +3065,7 @@ extern "C" int jb200_stream_restart(jb200_decoder *d, int stream) {
     JB_RC(reset_slots(d, stream, 1));
     JB_CUDA(cudaStreamSynchronize(d->stream));
   }
-  d->st_t[stream] = 0; d->st_started[stream] = 0; d->st_done[stream] = 0; d->st_in[stream] = 0;
+  d->st_t[stream] = 0; d->st_started[stream] = 0; d->st_done[stream] = 0; d->in.st_in[stream] = 0;
   return JB200_OK;
 }
 
@@ -3021,5 +3132,239 @@ extern "C" int jb200_decoder_frame_counts(jb200_decoder *d, int u, int32_t *coun
   const int f0 = d->h_frame_off[u], T = d->h_frame_off[u + 1] - f0;
   const int n = T < max_frames ? T : max_frames;
   JB_CUDA(cudaMemcpy(counts, d->P.counts + (size_t)f0 * 2, sizeof(int) * 2 * n, cudaMemcpyDeviceToHost));
+  return JB200_OK;
+}
+
+// ---- decoder groups (jb200_group_*): recognition instances on one acoustic model score each input once -------------
+struct jb200_group {
+  std::vector<jb200_decoder *> m;
+  std::vector<char> active;
+  std::vector<cudaEvent_t> beam_done;           // per member: its last beam over the group's rows, on its own stream
+  int device = 0;
+  RowSource in;                                 // the group's features, score rows and splice state
+  std::vector<void *> dev_allocs, host_allocs;  // freed by jb200_group_destroy
+  cudaStream_t stream = nullptr;
+  // ev[0..4]: upload begins, input on the device, scored, every member's beam done, results copied back
+  cudaEvent_t ev[5]{};
+  bool timed = false, fetched = false;
+  bool st_open = false; int st_n = 0;
+};
+
+extern "C" void jb200_group_destroy(jb200_group *g) {
+  if (!g) return;
+  cudaSetDevice(g->device);
+  // the members' beams may still read the group's rows
+  for (jb200_decoder *d : g->m) {
+    cudaStreamSynchronize(d->stream);
+    if (d->stream_group == g) d->stream_group = nullptr;
+  }
+  if (g->stream) cudaStreamSynchronize(g->stream);
+  for (void *p : g->dev_allocs) cudaFree(p);
+  for (void *p : g->host_allocs) cudaFreeHost(p);
+  for (auto &e : g->ev) if (e) cudaEventDestroy(e);
+  for (auto &e : g->beam_done) if (e) cudaEventDestroy(e);
+  if (g->stream) cudaStreamDestroy(g->stream);
+  delete g;
+}
+
+// the device half of jb200_group_create
+static int build_group(jb200_group *g) {
+  JB_CUDA(cudaSetDevice(g->device));
+  JB_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
+  for (auto &e : g->ev) JB_CUDA(cudaEventCreate(&e));
+  for (auto &e : g->beam_done) JB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  RowSource &s = g->in;
+  JB_RC(dev_alloc(g, (size_t)s.max_frames * s.dim, &s.d_feats));
+  JB_RC(dev_alloc(g, (size_t)s.max_frames * s.row_stride, &s.d_rows));
+  return reserve_splice(g, s, g->m[0]->in.ctx, g->m[0]->in.fl);
+}
+
+extern "C" int jb200_group_create(jb200_decoder *const *members, int n_members, jb200_group **out) {
+  if (!members || !out || n_members < 1 || n_members > JB200_GROUP_MAX) {
+    set_error("jb200_group_create: 1 to %d members", JB200_GROUP_MAX); return JB200_ERR_ARG;
+  }
+  const jb200_decoder *d0 = members[0];
+  for (int i = 0; i < n_members; i++) {
+    const jb200_decoder *d = members[i];
+    if (!d) { set_error("jb200_group_create: member %d is null", i); return JB200_ERR_ARG; }
+    for (int j = 0; j < i; j++)
+      if (members[j] == d) { set_error("jb200_group_create: members %d and %d are the same decoder", j, i); return JB200_ERR_ARG; }
+    if (d->in.am != d0->in.am || d->device != d0->device) {
+      set_error("jb200_group_create: member %d uses another acoustic model than member 0", i); return JB200_ERR_ARG;
+    }
+    if (d->in.dnn != d0->in.dnn) { set_error("jb200_group_create: member %d has another DNN than member 0", i); return JB200_ERR_ARG; }
+  }
+  jb200_group *g = new jb200_group();
+  g->m.assign(members, members + n_members);
+  g->active.assign(n_members, 1);
+  g->beam_done.assign(n_members, nullptr);
+  g->device = d0->device;
+  RowSource &s = g->in;
+  s.am = d0->in.am; s.dnn = d0->in.dnn; s.dim = d0->in.dim; s.S = d0->in.S; s.row_stride = d0->in.row_stride;
+  s.max_utts = d0->max_utts; s.max_frames = d0->max_frames;
+  for (const jb200_decoder *d : g->m) { s.max_utts = std::min(s.max_utts, d->max_utts); s.max_frames = std::min(s.max_frames, d->max_frames); }
+  const int rc = build_group(g);
+  if (rc) { jb200_group_destroy(g); return rc; }
+  *out = g;
+  return JB200_OK;
+}
+
+extern "C" int jb200_group_set_active(jb200_group *g, int member, int active) {
+  if (!g || member < 0 || member >= (int)g->m.size()) { set_error("jb200_group_set_active: bad argument"); return JB200_ERR_ARG; }
+  // a stream that missed feeds, or got feeds its member did not, cannot go on: the change waits for the utterances' ends
+  const jb200_decoder *d = g->m[member];
+  if (g->st_open && (g->active[member] != 0) != (active != 0) && d->stream_group == g)
+    for (int u = 0; u < d->st_n; u++)
+      if (d->st_started[u] && !d->st_done[u]) {
+        set_error("jb200_group_set_active: member %d is inside an utterance on stream %d; end or restart it first", member, u);
+        return JB200_ERR_ARG;
+      }
+  g->active[member] = active ? 1 : 0;
+  return JB200_OK;
+}
+
+// The start of a group call, once it has been checked: the group's stream waits (on the device) until no member's beam
+// of an earlier call still reads the rows, then ev[0]
+static int group_begin(jb200_group *g) {
+  JB_CUDA(cudaSetDevice(g->device));
+  for (cudaEvent_t e : g->beam_done) JB_CUDA(cudaStreamWaitEvent(g->stream, e, 0));
+  JB_CUDA(cudaEventRecord(g->ev[0], g->stream));
+  g->timed = true; g->fetched = false;
+  return JB200_OK;
+}
+
+// Once the rows are scored (ev[2] on the group's stream): every active member's beam waits for them on its own stream.
+// launch(i) launches member i's beam and tells whether it did; ev[3] follows the last of them.
+template <typename Launch>
+static int group_beams(jb200_group *g, Launch launch) {
+  JB_CUDA(cudaEventRecord(g->ev[2], g->stream));
+  for (size_t i = 0; i < g->m.size(); i++) {
+    if (!g->active[i]) continue;
+    jb200_decoder *d = g->m[i];
+    JB_CUDA(cudaStreamWaitEvent(d->stream, g->ev[2], 0));
+    JB_RC(launch(i));
+    JB_CUDA(cudaEventRecord(g->beam_done[i], d->stream));
+    JB_CUDA(cudaStreamWaitEvent(g->stream, g->beam_done[i], 0));
+  }
+  JB_CUDA(cudaEventRecord(g->ev[3], g->stream));
+  return JB200_OK;
+}
+
+// ev[4] after the results of the active members have been copied back
+static int group_fetched(jb200_group *g) {
+  JB_CUDA(cudaEventRecord(g->ev[4], g->stream));
+  g->fetched = true;
+  return JB200_OK;
+}
+
+static int group_batch(jb200_group *g, BatchInput in, const float *x, const int32_t *frame_off, int n_utts) {
+  if (!g) { set_error("null group"); return JB200_ERR_ARG; }
+  RowSource &s = g->in;
+  std::vector<int32_t> rows_off;
+  const int32_t *rows = nullptr;
+  JB_RC(batch_rows_off(s, in, x, frame_off, n_utts, rows_off, &rows));
+  JB_RC(check_batch(s, rows, n_utts));          // the group's capacity is the smallest member's
+  for (jb200_decoder *d : g->m) if (d->stream_group == g) d->stream_group = nullptr;
+  g->st_open = false;
+  for (size_t i = 0; i < g->m.size(); i++) if (g->active[i]) JB_RC(prepare_batch(g->m[i], rows, n_utts, false));
+  if (rows != frame_off) {
+    JB_CUDA(cudaSetDevice(g->device));
+    JB_CUDA(cudaStreamSynchronize(g->stream));  // the staging segment table may still feed the last call's copy
+  }
+  JB_RC(group_begin(g));
+  const float *d_x = nullptr;
+  JB_RC(batch_rows(s, g->stream, in, x, frame_off, rows, n_utts, g->ev[1], true, &d_x));
+  JB_RC(group_beams(g, [&](size_t i) {
+    // the member's own timing: no upload or scoring of its own, then its beam
+    jb200_decoder *d = g->m[i];
+    for (int k = 0; k < 3; k++) JB_CUDA(cudaEventRecord(d->ev[k], d->stream));
+    JB_RC(launch_beam(d, n_utts, 0, 0, s.d_rows));
+    if (in == FEATS_DEVICE) JB_CUDA(cudaEventRecord(d->ev[3], d->stream));
+    return JB200_OK;
+  }));
+  if (in == FEATS_DEVICE) return JB200_OK;
+  for (size_t i = 0; i < g->m.size(); i++) if (g->active[i]) JB_RC(jb200_decoder_fetch(g->m[i]));
+  return group_fetched(g);
+}
+
+extern "C" int jb200_group_decode_batch_host(jb200_group *g, const float *feats, const int32_t *frame_off, int n_utts) {
+  return group_batch(g, FEATS_HOST, feats, frame_off, n_utts);
+}
+
+extern "C" int jb200_group_decode_batch_device(jb200_group *g, const float *d_feats, const int32_t *frame_off, int n_utts) {
+  return group_batch(g, FEATS_DEVICE, d_feats, frame_off, n_utts);
+}
+
+extern "C" int jb200_group_decode_batch_scores_host(jb200_group *g, const float *scores, const int32_t *frame_off, int n_utts) {
+  return group_batch(g, SCORES_HOST, scores, frame_off, n_utts);
+}
+
+extern "C" int jb200_group_stream_open(jb200_group *g, int n_streams) {
+  if (!g || n_streams < 1) { set_error("jb200_group_stream_open: bad argument"); return JB200_ERR_ARG; }
+  if (n_streams > g->in.max_utts) { set_error("%d streams exceed group capacity %d", n_streams, g->in.max_utts); return JB200_ERR_CAPACITY; }
+  g->st_open = false;
+  for (jb200_decoder *d : g->m) {
+    JB_RC(jb200_stream_open(d, n_streams));
+    d->stream_group = g;
+  }
+  g->in.st_in.assign(n_streams, 0);
+  g->st_open = true; g->st_n = n_streams;
+  return JB200_OK;
+}
+
+extern "C" int jb200_group_stream_restart(jb200_group *g, int stream) {
+  if (!g || !g->st_open || stream < 0 || stream >= g->st_n) { set_error("jb200_group_stream_restart: bad argument"); return JB200_ERR_ARG; }
+  for (size_t i = 0; i < g->m.size(); i++)
+    if (g->active[i] && g->m[i]->stream_group == g) JB_RC(jb200_stream_restart(g->m[i], stream));
+  g->in.st_in[stream] = 0;
+  return JB200_OK;
+}
+
+static int group_feed(jb200_group *g, bool scores, const float *x, const int32_t *n_new, const uint8_t *last, int want_interim) {
+  if (!g || !n_new) { set_error("jb200_group_stream_feed: bad argument"); return JB200_ERR_ARG; }
+  if (!g->st_open) { set_error("jb200_group_stream_feed: call jb200_group_stream_open first"); return JB200_ERR_ARG; }
+  for (size_t i = 0; i < g->m.size(); i++) {
+    const jb200_decoder *d = g->m[i];
+    if (g->active[i] && (d->stream_group != g || !d->stream_mode)) {
+      set_error("jb200_group_stream_feed: member %zu has left the group's stream", i); return JB200_ERR_ARG;
+    }
+  }
+  RowSource &s = g->in;
+  std::vector<int32_t> rows;
+  JB_RC(feed_rows(s, scores, n_new, g->st_n, rows));
+  for (size_t i = 0; i < g->m.size(); i++) if (g->active[i]) JB_RC(check_feed(g->m[i], n_new, rows.data()));
+  JB_RC(feed_totals(s, scores, x, n_new, rows.data(), g->st_n));
+  JB_RC(group_begin(g));
+  JB_RC(feed_score(s, g->stream, scores, x, n_new, rows.data(), g->st_n, g->ev[1]));
+  std::vector<char> launched(g->m.size(), 0);
+  JB_RC(group_beams(g, [&](size_t i) {
+    bool l = false;
+    JB_RC(stream_launch(g->m[i], rows.data(), last, want_interim, s.d_rows, &l));
+    launched[i] = l;
+    return JB200_OK;
+  }));
+  for (size_t i = 0; i < g->m.size(); i++) if (launched[i]) JB_RC(stream_collect(g->m[i]));
+  return group_fetched(g);
+}
+
+extern "C" int jb200_group_stream_feed_host(jb200_group *g, const float *feats, const int32_t *n_new, const uint8_t *last, int want_interim) {
+  return group_feed(g, false, feats, n_new, last, want_interim);
+}
+
+extern "C" int jb200_group_stream_feed_scores_host(jb200_group *g, const float *scores, const int32_t *n_new, const uint8_t *last, int want_interim) {
+  return group_feed(g, true, scores, n_new, last, want_interim);
+}
+
+extern "C" int jb200_group_last_timing(jb200_group *g, float ms[4]) {
+  if (!g || !ms) { set_error("bad argument"); return JB200_ERR_ARG; }
+  for (int i = 0; i < 4; i++) ms[i] = 0.0f;
+  if (!g->timed) return JB200_OK;
+  JB_CUDA(cudaSetDevice(g->device));
+  JB_CUDA(cudaEventSynchronize(g->ev[3]));
+  for (int i = 0; i < 3; i++) JB_CUDA(cudaEventElapsedTime(&ms[i], g->ev[i], g->ev[i + 1]));
+  if (g->fetched) {
+    JB_CUDA(cudaEventSynchronize(g->ev[4]));
+    JB_CUDA(cudaEventElapsedTime(&ms[3], g->ev[3], g->ev[4]));
+  }
   return JB200_OK;
 }

@@ -288,6 +288,9 @@ struct jb200_dnn {
   int cap_frames = 0, max_width = 0, ld_logits = 0, n_sm = 0;
   float *d_in = nullptr, *d_logits = nullptr, *d_rows = nullptr;
   __nv_bfloat16 *act_hi[2] = {nullptr, nullptr}, *act_lo[2] = {nullptr, nullptr};
+  // the end of the last forward: the next one waits for it on its own stream, since every forward uses the buffers above
+  // and decoders (or a decoder group) sharing the handle call it on different streams
+  cudaEvent_t forward_done = nullptr;
 };
 
 static int make_map(jb200_dnn *h, CUtensorMap *map, void *base, int rows, int cols_ld, int cols_valid) {
@@ -308,6 +311,7 @@ extern "C" void jb200_dnn_destroy(jb200_dnn *h) {
   for (auto &l : h->L) { cudaFree(l.w_hi); cudaFree(l.w_lo); cudaFree(l.bias); }
   cudaFree(h->d_prior); cudaFree(h->d_logistic); cudaFree(h->d_addlog); cudaFree(h->d_in); cudaFree(h->d_logits); cudaFree(h->d_rows);
   for (int i = 0; i < 2; i++) { cudaFree(h->act_hi[i]); cudaFree(h->act_lo[i]); }
+  if (h->forward_done) cudaEventDestroy(h->forward_done);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -429,6 +433,8 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
   if (T <= 0) return JB200_OK;
   JB_CUDA(cudaSetDevice(h->device));
   int rc = dnn_reserve(h, T); if (rc) return rc;
+  if (!h->forward_done) JB_CUDA(cudaEventCreateWithFlags(&h->forward_done, cudaEventDisableTiming));
+  JB_CUDA(cudaStreamWaitEvent(st, h->forward_done, 0));
   int cur = 0;
   {
     const int ld = h->L[0].ld_in;
@@ -455,6 +461,7 @@ int dnn_forward_device(jb200_dnn *h, const float *d_in, int T, float *d_rows, in
   dnn_softmax_kernel<<<(T + 32 * SOFTMAX_WARPS - 1) / (32 * SOFTMAX_WARPS), 32 * SOFTMAX_WARPS, 0, st>>>(h->d_logits, h->ld_logits, h->out_dim, T,
                                                                                         h->d_prior, h->d_addlog, d_rows, row_stride);
   JB_LAUNCH_CHECK();
+  JB_CUDA(cudaEventRecord(h->forward_done, st));
   return JB200_OK;
 }
 }  // namespace jb200
