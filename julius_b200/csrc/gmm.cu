@@ -155,9 +155,11 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
       float res[GMM_FPT];
       if (!PRUNE) {
         // streaming log-add from the LAST mixture down to the first (addlog.c:108-121)
+        // FAST: the running sum starts from addlog_array's seed, a term at LOG_ZERO (y = LOG_ZERO, ssum = 1).  It vanishes
+        // (expf underflows) unless every term lies within ~88 of LOG_ZERO, e.g. a state whose densities are all NULL
         float y[GMM_FPT], ssum[GMM_FPT];
 #pragma unroll
-        for (int k = 0; k < GMM_FPT; k++) { y[k] = JB200_LOG_ZERO; ssum[k] = 0.0f; }
+        for (int k = 0; k < GMM_FPT; k++) { y[k] = JB200_LOG_ZERO; ssum[k] = 1.0f; }
         for (int m = nm - 1; m >= 0; m--) {
           const float4 *p = reinterpret_cast<const float4 *>(pb + (size_t)(grel + m) * STRIDE);
           const float gconst = pb[(size_t)(grel + m) * STRIDE + rec_gconst(D)];
@@ -229,12 +231,15 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
               float x = __fsub_rn(v[k][d], rec[rec_mean(d)]);
               acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(x, x), rec[rec_ivar(d)]));
             }
-            float sc = (gconst != gconst) ? JB200_LOG_ZERO : acc * -0.5f;
+            // compute_g_safe gives up (LOG_ZERO) as soon as its partial sum passes thres * -2; the partial sums never
+            // decrease, so that is the full sum passing it.  Such a LOG_ZERO is kept when thres itself is below LOG_ZERO.
+            float sc = (gconst != gconst) ? JB200_LOG_ZERO
+                     : (num >= gprune_num && acc > thres * -2.0f) ? JB200_LOG_ZERO : acc * -0.5f;
             if (num >= gprune_num && sc <= thres) continue;
             num = cache_push_dev(cs, ci, gprune_num, m, sc, num);
             thres = cs[num - 1];
           }
-          float y = JB200_LOG_ZERO, ssum = 0.0f;
+          float y = JB200_LOG_ZERO, ssum = 1.0f;   // seeded as above
           for (int i = num - 1; i >= 0; i--) {
             float sc = __fadd_rn(cs[i], pb[(size_t)(grel + ci[i]) * STRIDE + rec_lnw(D)]);
             if (EXACT) y = addlog_step_exact(y, sc, tbl);
@@ -364,13 +369,18 @@ static int gmm_build(jb200_gmm *h, const jb200_gmm_desc *d, const std::vector<in
     rec[rec_gconst(h->D)] = d->valid[g] ? d->gconst[g] : NAN;
     rec[rec_lnw(h->D)] = d->lnweight[g];
   }
-  // tiles: consecutive states, <= GMM_TILE_STATES states and <= GMM_TILE_GAUSS Gaussians
+  // tiles: consecutive states, <= GMM_TILE_STATES states with mixtures and <= GMM_TILE_GAUSS Gaussians.  States without
+  // mixtures ride along beyond the state cap, so every state is in a tile and gets its column written (LOG_ZERO); a tile
+  // closes only at a state with mixtures that does not fit, which then opens the next one.  The kernel's state loop has
+  // no bound of its own.  A tile without Gaussians is left out: it arises only when the model has none.
   std::vector<GmmTile> tiles;
   for (int s = 0; s < h->S;) {
     GmmTile t{s, 0, (h->G > 0) ? d->state_off[s] : 0, 0};
-    while (s < h->S && t.ns < GMM_TILE_STATES && t.ng + mixcnt[s] <= GMM_TILE_GAUSS) { t.ng += mixcnt[s]; t.ns++; s++; }
+    int filled = 0;   // states with mixtures in t
+    while (s < h->S && (mixcnt[s] == 0 || (filled < GMM_TILE_STATES && t.ng + mixcnt[s] <= GMM_TILE_GAUSS))) {
+      t.ng += mixcnt[s]; t.ns++; filled += mixcnt[s] > 0; s++;
+    }
     if (t.ng > 0) tiles.push_back(t);
-    else if (t.ns == 0) s++;   // cannot happen (mixcnt<=TILE_GAUSS)
   }
   h->n_tiles = (int)tiles.size();
   size_t tile_bytes = tiles.size() * sizeof(GmmTile) + mixcnt.size() * sizeof(int);
@@ -401,6 +411,9 @@ extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, j
     set_error("-tmix %d outside supported range 1..%d", d->gprune_num, GMM_NMAX); return JB200_ERR_UNSUPPORTED;
   }
   if (d->iwcd_method == JB200_IWCD_NBEST && d->iwcd_nbest > GMM_NMAX) { set_error("-iwcd1 best %d too large", d->iwcd_nbest); return JB200_ERR_UNSUPPORTED; }
+  if (d->n_gauss > 0 && d->dim != 39 && d->dim != 38 && d->dim != 26 && d->dim != 25) {
+    set_error("feature dimension %d not instantiated (39, 38, 26, 25)", d->dim); return JB200_ERR_UNSUPPORTED;
+  }
   std::vector<int> mixcnt(d->n_states);
   for (int s = 0; s < d->n_states; s++) {
     mixcnt[s] = (d->n_gauss > 0) ? d->state_off[s + 1] - d->state_off[s] : 0;

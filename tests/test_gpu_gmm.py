@@ -2,8 +2,8 @@
 import numpy as np
 import pytest
 
-from julius_b200 import capi
-from util import CASES, Golden, rel_err
+from julius_b200 import capi, desc
+from util import CASES, GMM_DIMS, Golden, random_frames, random_gmm, random_gmm_counts, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -47,13 +47,11 @@ def test_ragged_and_tiny_batches(oracle_lib):
         assert np.array_equal(out, g.utts[0].outprob[:T])
 
 
-def test_gauss_hook_contract(oracle_lib):
-    """calcmix contract: per-Gaussian ln scores without mixture weight (plugin/calcmix.c:226-323)."""
-    g = Golden("tiny")
-    sc = capi.GmmScorer(g.ds, mode=capi.GMM_EXACT)
-    x = g.feats[0][7]
+def _check_gauss_hook(b, ds, x):
+    """the device's per-Gaussian scores of frame x against a float32 loop in the reference's statement order; a NULL
+    density scores LOG_ZERO"""
+    sc = capi.GmmScorer(ds, mode=capi.GMM_EXACT)
     got = sc.gauss(x)
-    b = g.blob
     D = b["gmm.dim"][0]
     mean = b["gmm.mean"].reshape(-1, D); iv = b["gmm.ivar"].reshape(-1, D)
     want = np.empty(len(mean), np.float32)
@@ -62,8 +60,22 @@ def test_gauss_hook_contract(oracle_lib):
         for d in range(D):
             xx = np.float32(x[d] - mean[k, d])
             tmp = np.float32(tmp + np.float32(np.float32(xx * xx) * iv[k, d]))
-        want[k] = np.float32(tmp * np.float32(-0.5))
+        want[k] = np.float32(tmp * np.float32(-0.5)) if b["gmm.valid"][k] else np.float32(-1e6)
     assert np.array_equal(got, want)
+
+
+def test_gauss_hook_contract(oracle_lib):
+    """calcmix contract: per-Gaussian ln scores without mixture weight (plugin/calcmix.c:226-323)."""
+    g = Golden("tiny")
+    _check_gauss_hook(g.blob, g.ds, g.feats[0][7])
+
+
+@pytest.mark.parametrize("dim", GMM_DIMS)
+def test_gauss_hook_contract_at_each_dimension(dim):
+    """the same contract on a ragged random model with NULL densities at each dimension K1 is built for"""
+    blob = random_gmm(random_gmm_counts(dim), dim, seed=dim)
+    assert (blob["gmm.valid"] == 0).any()
+    _check_gauss_hook(blob, desc.Descriptors(blob), random_frames(dim, 1, seed=dim, n_far=0)[0])
 
 
 def test_large_batch_linearity_property():

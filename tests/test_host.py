@@ -179,8 +179,8 @@ def test_dnn_create_refuses_inconsistent_widths():
 
 
 def test_gmm_create_refuses_unsupported_descriptors():
-    """jb200_gmm_create checks -tmix, -iwcd1 best and the mixtures per state before it looks for a device: each is
-    JB200_ERR_UNSUPPORTED, with or without a GPU."""
+    """jb200_gmm_create checks -tmix, -iwcd1 best, the mixtures per state and the feature dimension (25, 26, 38 or 39
+    when the model has Gaussians) before it looks for a device: each is JB200_ERR_UNSUPPORTED, with or without a GPU."""
     g = Golden("tiny")
     too_many_mix = g.blob["gmm.state_off"].copy()
     too_many_mix[1] = too_many_mix[0] + 65
@@ -198,6 +198,8 @@ def test_gmm_create_refuses_unsupported_descriptors():
     assert create(g.blob, gprune_method=1, gprune_num=0) == -4               # -tmix 0 with pruning on
     assert create(g.blob, iwcd_method=2, iwcd_nbest=17) == -4                # -iwcd1 best 17
     assert create(dict(g.blob, **{"gmm.state_off": too_many_mix})) == -4     # a state with 65 mixtures
+    assert create(g.blob, dim=13) == -4                                      # a feature dimension K1 is not built for
+    assert create(g.blob, dim=13, n_gauss=0) in (0, -3)                      # cd sets only: the dimension is not used
     assert create(g.blob) in (0, -3)                                         # JB200_OK, or JB200_ERR_NODEVICE without a GPU
 
 

@@ -212,6 +212,207 @@ def single_layer_scores_np(blob, x, tbl):
     return out.astype(np.float32)
 
 
+# ---- designed GMMs (tests/test_gmm_design.py, tests/test_gpu_gmm_shapes.py) -----------------------------------------
+# K1 is instantiated for these feature dimensions; even ones keep gconst / ln w in an extra quad of the record.
+GMM_DIMS = [25, 26, 38, 39]
+LOG_ZERO = np.float32(-1000000.0)
+LOG_ADDMIN = -13.815510558                        # a double: the drop test compares a float difference with it
+ADDMIN_KEPT = np.float32(np.nextafter(np.float32(LOG_ADDMIN), np.float32(0)))
+if float(ADDMIN_KEPT) < LOG_ADDMIN:               # the float just above LOG_ADDMIN, whichever way the cast rounded
+    ADDMIN_KEPT = np.nextafter(ADDMIN_KEPT, np.float32(0))
+ADDMIN_DROPPED = np.nextafter(ADDMIN_KEPT, np.float32(-np.inf))   # the float just below it
+TILE_STATES, TILE_GAUSS = 4, 64                   # K1's tile caps (gmm.cu)
+
+# mixture counts in tiling order: empty states at the start, a tile ending at exactly 64 Gaussians, a 64-mixture state,
+# 65 Gaussians (40 + 25: a split), empty states right after a full 4-state tile (a run of 1 and a run of 4), a single
+# empty state in the middle, more than 4 one-mixture states, ragged counts, empty states at the end after a full tile
+TILING_PATTERN = ([0, 0, 3, 61, 64, 8, 8, 8, 8, 0, 40, 25, 39, 8, 8, 8, 8, 0, 0, 0, 0, 8, 5, 0, 7] + [1] * 9
+                  + [20, 20, 24, 2, 0, 1, 16])
+TILING_TAIL = [8, 8, 8, 8, 0]
+# the two examples of states no tile used to cover
+EMPTY_STATE_PATTERNS = {"4full_then_1empty": [8, 8, 8, 8, 0], "4full_4empty_8": [8, 8, 8, 8, 0, 0, 0, 0, 8]}
+
+
+def gmm_tiles(counts):
+    """K1's tiling (gmm_build) in Python: [(first state, states, Gaussians)]"""
+    tiles, s, S = [], 0, len(counts)
+    while s < S:
+        s0, ng, filled = s, 0, 0
+        while s < S and (counts[s] == 0 or (filled < TILE_STATES and ng + counts[s] <= TILE_GAUSS)):
+            ng += counts[s]
+            filled += counts[s] > 0
+            s += 1
+        if ng > 0:
+            tiles.append((s0, s - s0, ng))
+    return tiles
+
+
+def tiles_per_cta(T, n_tiles, sms):
+    """the tiles one CTA of K1 walks for T frames (launch_gmm: about 8 CTAs per SM)"""
+    fblocks = -(-T // 256)
+    chunks = min(max(1, -(-sms * 8 // fblocks)), n_tiles)
+    return -(-n_tiles // chunks)
+
+
+def gmm_blob(counts, dim, mean, ivar, gconst, lnw, valid, cdsets=(), iwcd=(2, 3), gprune=(0, 2)):
+    """A GMM blob dict (the entries desc.Descriptors reads) from per-state mixture counts, per-Gaussian parameters and
+    pseudo-phone (cd) sets given as lists of member states."""
+    counts = np.asarray(counts, np.int64)
+    off = np.zeros(len(counts) + 1, np.int32)
+    np.cumsum(counts, out=off[1:])
+    G = int(off[-1])
+    cd_off = np.zeros(len(cdsets) + 1, np.int32)
+    np.cumsum([len(c) for c in cdsets], out=cd_off[1:])
+    cd_states = np.array([s for c in cdsets for s in c], np.int32)
+    i32 = lambda v: np.array([v], np.int32)
+    return {"gmm.n_states": i32(len(counts)), "gmm.dim": i32(dim), "gmm.n_gauss": i32(G),
+            "gmm.max_mix": i32(max(1, int(counts.max(initial=0)))), "gmm.gprune_method": i32(gprune[0]),
+            "gmm.gprune_num": i32(gprune[1]), "gmm.state_off": off,
+            "gmm.mean": np.ascontiguousarray(mean, np.float32).reshape(G * dim),
+            "gmm.ivar": np.ascontiguousarray(ivar, np.float32).reshape(G * dim),
+            "gmm.gconst": np.ascontiguousarray(gconst, np.float32), "gmm.lnweight": np.ascontiguousarray(lnw, np.float32),
+            "gmm.valid": np.ascontiguousarray(valid, np.uint8),
+            "am.iwcd_method": i32(iwcd[0]), "am.iwcd_nbest": i32(iwcd[1]), "am.n_cdsets": i32(len(cdsets)),
+            "am.n_cdset_states": i32(len(cd_states)), "am.cd_off": cd_off, "am.cd_states": cd_states}
+
+
+def random_gmm_counts(seed, n_ragged=300):
+    rng = np.random.default_rng(seed)
+    return TILING_PATTERN + rng.integers(1, 17, n_ragged).tolist() + TILING_TAIL
+
+
+def cdset_designs(counts, rng):
+    """cd sets over a model's states: 1 member, 2..17 members (below, at and above every best N), 24 and 40 members,
+    sets with a repeated member (tied scores), sets holding empty (LOG_ZERO) states and a set of empty states only"""
+    counts = np.asarray(counts)
+    full, empty = np.nonzero(counts > 0)[0], np.nonzero(counts == 0)[0]
+    pick = lambda n: rng.choice(full, n, replace=n > len(full)).tolist()
+    sets = [pick(n) for n in [1, 2, 3, 4, 5, 6, 7, 8, 9, 15, 16, 17, 24, 40]]
+    for n in (3, 5, 9, 17):
+        m = pick(n - 1)
+        sets.append(m + [m[n // 2]])                                       # a tie
+        sets.append(m[:n // 2] + [int(empty[0])] + m[n // 2:])             # a member at LOG_ZERO
+    sets.append([int(e) for e in empty[:3]])                               # all LOG_ZERO: 0/0 in AVG and best N
+    return sets
+
+
+def random_gmm(counts, dim, seed, null_frac=0.1):
+    """Means N(0,1), inverse variances in [0.2, 5] with their gconst, Dirichlet weights, about null_frac NULL densities,
+    one 8-mixture state with all densities NULL and states with a NULL first, last, and first and last mixture."""
+    rng = np.random.default_rng(seed)
+    counts = list(counts)
+    G = int(sum(counts))
+    mean = rng.standard_normal((G, dim)).astype(np.float32)
+    ivar = rng.uniform(0.2, 5.0, (G, dim)).astype(np.float32)
+    gconst = (dim * np.log(2 * np.pi) - np.log(ivar.astype(np.float64)).sum(1)).astype(np.float32)
+    lnw = np.concatenate([np.log(rng.dirichlet(np.full(c, 2.0))) for c in counts if c > 0]).astype(np.float32)
+    valid = (rng.random(G) >= null_frac).astype(np.uint8)
+    off = np.concatenate([[0], np.cumsum(counts)])
+    eight = [s for s, c in enumerate(counts) if c == 8]
+    valid[off[eight[0]]:off[eight[0] + 1]] = 0
+    big = [s for s, c in enumerate(counts) if c >= 12]
+    valid[off[big[0]]] = 0
+    valid[off[big[1] + 1] - 1] = 0
+    valid[off[big[2]]] = valid[off[big[2] + 1] - 1] = 0
+    return gmm_blob(counts, dim, mean, ivar, gconst, lnw, valid, cdset_designs(counts, rng))
+
+
+def random_frames(dim, T, seed, n_far=32):
+    """features N(0, 1.2), then n_far far frames (scale 30 .. 3000) whose Gaussian sums cross LOG_ZERO"""
+    rng = np.random.default_rng(seed)
+    x = rng.normal(0.0, 1.2, (T, dim))
+    x[T - n_far:] *= np.geomspace(25.0, 2500.0, n_far)[:, None]
+    return x.astype(np.float32)
+
+
+def index_rounding_diffs(n_each=4):
+    """differences d (floats in (LOG_ADDMIN, 0)) whose table index (double)(-d) * 33333.3333 + 0.5 lies within a few
+    float ulps below / above an integer, picked where the same index taken in float arithmetic lands on the other side"""
+    d = -np.float32(np.linspace(0.5, 13.5, 2_000_003)).astype(np.float32)
+    r = (-d).astype(np.float64) * 33333.3333 + 0.5
+    i_d = r.astype(np.int64)
+    i_mul = (np.float32(-d) * np.float32(33333.3333) + np.float32(0.5)).astype(np.int64)
+    i_fma = ((-d).astype(np.float64) * np.float64(np.float32(33333.3333)) + 0.5).astype(np.float32).astype(np.int64)
+    frac = r - np.rint(r)
+    near = np.abs(frac) < 4 * np.spacing(r.astype(np.float32)).astype(np.float64)
+    pick = []
+    for side in (frac < 0, frac > 0):
+        idx = np.nonzero(near & side & (i_d != i_mul) & (i_d != i_fma))[0]
+        pick += idx[np.linspace(0, len(idx) - 1, n_each).astype(int)].tolist()
+    return d[pick]
+
+
+def addlog_designs():
+    """{name: weighted terms} for states with ivar = 0, where every term is exactly gconst * -0.5 + ln w (ln w = 0)"""
+    rng = np.random.default_rng(5)
+    f = lambda *v: np.array(v, np.float32)
+    d = {"addmin_kept": f(-1.5, np.float32(-1.5) + ADDMIN_KEPT), "addmin_dropped": f(-1.5, np.float32(-1.5) + ADDMIN_DROPPED),
+         "addmin_kept_rev": f(np.float32(-1.5) + ADDMIN_KEPT, -1.5),
+         "equal64": np.full(64, -3.0, np.float32),
+         "peak_first": np.concatenate([[4.0], rng.normal(-6, 2, 11)]).astype(np.float32),
+         "peak_last": np.concatenate([rng.normal(-6, 2, 11), [4.0]]).astype(np.float32),
+         "below_log_zero": f(-2e6, -1.5e6, -3e6), "at_log_zero": f(-1e6), "near_log_zero": f(-1000003.0, -1000001.0),
+         "exact_zero": f(0.0), "exact_zero_2": f(0.0, -20.0)}
+    for i, x in enumerate(index_rounding_diffs()):
+        d[f"index_{i}"] = f(0.0, x)
+    return d
+
+
+EXACT_ZERO_DESIGNS = ("exact_zero", "exact_zero_2")
+
+
+def prune_designs(n):
+    """{name: (scores, ln w, kept list)} for -tmix n: the kept list is the top-n list the pruned walk must end with, in
+    list order (best first).  Scores are 0.25-grid values; the weights make every kept id visible in the sum."""
+    w = lambda k: np.log(np.arange(1, k + 1, dtype=np.float64) / (k * (k + 1) / 2))
+    highs = [6.0 + i for i in range(max(n - 2, 0))][::-1]
+    d = {}
+    # a later equal score goes in front of an earlier one; the next insertion then drops the earlier one
+    if n >= 2:
+        sc = highs + [4.0, 3.0, 4.0, 4.5]
+        k = len(highs)
+        d["tie_order"] = (sc, w(len(sc)), list(range(k)) + [k + 3, k + 2])
+    # a candidate equal to the n-th best is dropped
+    sc = [5.0 + i for i in range(n)][::-1] + [5.0]
+    d["equal_nth"] = (sc, w(len(sc))[::-1], list(range(n)))
+    # equal scores: the first n mixtures stay, whatever their weights
+    d["equal_scores"] = ([-2.0] * (n + 3), w(n + 3)[::-1], list(range(n)))
+    # fewer mixtures than -tmix
+    d["fewer_than_tmix"] = ([1.0, 3.0], w(2), [1, 0][:n])
+    return {k: (np.array(s, np.float32), np.array(l, np.float32), kept) for k, (s, l, kept) in d.items()}
+
+
+def design_gmm(dim, seed, tmix=None):
+    """A model with one state per addlog design (ln w = 0), and with tmix the prune designs for -tmix tmix, separated by
+    empty states; ivar = 0 so that each Gaussian's log-likelihood is gconst * -0.5 on every frame.
+    -> (blob, [state name or None for an empty state])"""
+    rng = np.random.default_rng(seed)
+    states = [(k, v, np.zeros(len(v), np.float32)) for k, v in addlog_designs().items()]
+    if tmix is not None:
+        states += [(k, s, l) for k, (s, l, _) in prune_designs(tmix).items()]
+    names, counts, scores, lnws = [], [], [], []
+    for i, (k, s, l) in enumerate(states):
+        if i % 3 == 0:
+            names.append(None); counts.append(0)
+        names.append(k); counts.append(len(s)); scores.append(s); lnws.append(l)
+    names.append(None); counts.append(0)
+    sc = np.concatenate(scores)
+    G = len(sc)
+    gconst = (sc * np.float32(-2.0)).astype(np.float32)
+    assert np.array_equal(gconst * np.float32(-0.5), sc)
+    mean = rng.standard_normal((G, dim)).astype(np.float32)
+    blob = gmm_blob(counts, dim, mean, np.zeros((G, dim), np.float32), gconst, np.concatenate(lnws),
+                    np.ones(G, np.uint8), cdset_designs(counts, rng))
+    return blob, names
+
+
+def finish_np(lp):
+    """calc_mix.c:72-80 for one stream of weight 1 on float32 log-sums"""
+    lp = np.asarray(lp, np.float32)
+    out = (lp.astype(np.float64) * 0.434294482).astype(np.float32)
+    return np.where((lp <= LOG_ZERO) | (lp == 0), LOG_ZERO, out).astype(np.float32)
+
+
 # A golden model is stored whole (model.jb2m), or, where that file would exceed 1 MB, as model_delta.npz: the entries that
 # differ from the model of the golden case meta["base"] (all of them when there is no base), compressed; meta["drop"] lists
 # the base's entries the model does not have.
