@@ -5,7 +5,8 @@
 // (factoring_sub.c:942-1143, ngram_access.c:249-305) and the word-trellis store/sort
 // (backtrellis.c:190-267,438-478), stock "fast" switches: N-gram LMs on normal trees (beam_kernel<false, .>) and
 // multipath trees (beam_kernel_mp); DFA grammars on the category tree (beam_kernel<true, .> = the same body with the
-// three grammar-mode differences compiled in).
+// three grammar-mode differences compiled in).  outprob_style's pseudo-phone set score is outprob_cd in common.cuh, the
+// same code that fills the cd-set columns of the scorer's rows.
 //
 // Why this is not a transliteration.  The reference walks the survivors of frame t-1 one by one
 // and lets each arc "propagate" into a per-node slot; ties are won by whoever arrived first, new
@@ -46,13 +47,12 @@ int gmm_device(const jb200_gmm *h);
 int gmm_dim(const jb200_gmm *h);
 int gmm_launch_states(jb200_gmm *h, const float *d_feats, int T, float *d_rows, int row_stride, cudaStream_t st,
                       const int *seg_off, const int *seg_start, int n_seg);
-int gmm_cd_device(const jb200_gmm *h, const int **cd_off, const int **cd_states, int *method, int *nbest);
+CdSets gmm_cdsets(const jb200_gmm *h);
 
 static constexpr int BEAM_THREADS = 256;
 static constexpr int NWARP = BEAM_THREADS / 32;
 static constexpr int SEQ_LOCAL_BITS = 18;
 static constexpr unsigned SEQ_LOCAL = 1u << SEQ_LOCAL_BITS;
-static constexpr int CD_NMAX = 16;
 static constexpr int MAX_WORDS = 150;      // MAXSEQNUM, libsent/include/sent/speech.h:50
 
 struct __align__(16) NodeRec { float self_a, next_a; int arc_off, arc_n; int stend, next; int scid, out; };   // 32 B; (scid,out) is one aligned 8-byte word; next = the node next_a leads to
@@ -121,7 +121,7 @@ struct BeamParams {
   float lm_weight, lm_penalty, lm_penalty_trans, prune_width;
   int head_node, tail_silwid, beam, n_nodes;
   // cd sets
-  const int *cd_off; const int *cd_states; int iwcd_method, iwcd_nbest;
+  CdSets cd;
   // batch
   const float *rows; int row_stride; const int *frame_off;
   // per-utterance work areas (index = blockIdx.x)
@@ -205,71 +205,15 @@ __device__ __forceinline__ float max_successor_prob(const BeamParams &p, int las
   return v;
 }
 
-// outprob_cd, outprob.c:286-400, evaluated on demand from the frame's state-score row
-__device__ float cdset_score(const BeamParams &p, const float *__restrict__ row, int c) {
-  const int b0 = __ldg(p.cd_off + c), n_in = __ldg(p.cd_off + c + 1) - b0;
-  if (p.iwcd_method == JB200_IWCD_AVG) {
-    float sum = 0.0f; int j = 0;
-    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(p.cd_states + b0 + i)); if (v > JB200_LOG_ZERO) { sum += v; j++; } }
-    return sum / (float)j;
-  } else if (p.iwcd_method == JB200_IWCD_MAX) {
-    float mx = JB200_LOG_ZERO;
-    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(p.cd_states + b0 + i)); if (mx < v) mx = v; }
-    return mx;
-  }
-  const int maxn = p.iwcd_nbest;
-  if (maxn <= 3) {
-    // the kept list is the sorted multiset of the maxn largest valid scores, and the result adds it up from the
-    // largest down (outprob.c:313-318): three registers instead of an indexed array in local memory
-    float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY; int n = 0;
-    for (int i = 0; i < n_in; i++) {
-      const float v = __ldg(row + __ldg(p.cd_states + b0 + i));
-      if (v <= JB200_LOG_ZERO) continue;
-      n++;
-      if (v > m0) { m2 = m1; m1 = m0; m0 = v; }
-      else if (v > m1) { m2 = m1; m1 = v; }
-      else if (v > m2) m2 = v;
-    }
-    n = min(n, maxn);
-    float prob = 0.0f;
-    if (n > 0) prob += m0;
-    if (n > 1) prob += m1;
-    if (n > 2) prob += m2;
-    return prob / (float)n;
-  }
-  float mp[CD_NMAX + 1]; int n = 0;
-  for (int i = 0; i < n_in; i++) {
-    float prob = __ldg(row + __ldg(p.cd_states + b0 + i));
-    if (prob <= JB200_LOG_ZERO) continue;
-    if (n == 0 || prob <= mp[n - 1]) {
-      if (n == maxn) continue;
-      mp[n] = prob; n++;
-    } else {
-      for (int k = 0; k < n; k++) {
-        if (prob > mp[k]) {
-          int cnt = n - k - ((n == maxn) ? 1 : 0);
-          for (int q = k + cnt; q > k; q--) mp[q] = mp[q - 1];
-          mp[k] = prob;
-          break;
-        }
-      }
-      if (n < maxn) n++;
-    }
-  }
-  float prob = 0.0f;
-  for (int i = 0; i < n; i++) prob += mp[i];
-  return prob / (float)n;
-}
-
 // outprob_style, outprob_style.c:354-494 with the context resolution tabulated on the host
 __device__ __forceinline__ float outprob_style(const BeamParams &p, const float *__restrict__ row, int out, int last_wid) {
   const int style = (unsigned)out >> 28, ref = out & 0x0fffffff;
   if (style == JB200_AS_STATE) return __ldg(row + ref);
-  if (style == JB200_AS_LSET) return cdset_score(p, row, ref);
+  if (style == JB200_AS_LSET) return outprob_cd(p.cd, row, ref);
   const int col = (last_wid < 0) ? p.n_ctx : __ldg(p.word_ctx + last_wid);
   const int r = __ldg(p.rset_ctx + (size_t)ref * (p.n_ctx + 1) + col);
   if (r >= 0) return __ldg(row + r);
-  return cdset_score(p, row, -r - 1);
+  return outprob_cd(p.cd, row, -r - 1);
 }
 
 // block-wide exclusive scan of one int per thread; *total = block sum.  Ends with a barrier.
@@ -2372,7 +2316,7 @@ static int upload_lm(jb200_decoder *d, const jb200_tree_desc *t) {
   P.tail_silwid = t->tail_silwid; P.beam = t->beam_width;
   // cd sets come from the AM handle's descriptor: re-upload from the gmm handle is not exposed, so the
   // decoder asks the scorer for its device copies
-  gmm_cd_device(d->in.am, &P.cd_off, &P.cd_states, &P.iwcd_method, &P.iwcd_nbest);
+  P.cd = gmm_cdsets(d->in.am);
   // inter-word bigram rows for every last word (the reference's iw_sc_cache, fully populated)
   const int *d_iso_word = nullptr;
   JB_RC(dev_upload(d, t->iso_word, (size_t)t->n_iso, &d_iso_word));

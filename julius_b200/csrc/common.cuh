@@ -28,6 +28,67 @@ __device__ __forceinline__ float addlog_step_exact(float y, float x, const float
   return __fadd_rn(y, __ldg(tbl + idx));
 }
 
+// ---- outprob_cd (outprob.c:286-400): a pseudo-phone set's score from the frame's state-score row -------------------
+// The cd-set kernel fills the set columns with it and the beam kernels evaluate it on demand.  Plain + and / only: the
+// sums have no product to contract, and the beam kernels' machine code depends on the form.
+static constexpr int NBEST_MAX = 16;   // largest N of a best-N list: -iwcd1 best N, and -tmix N of the pruned K1 variants
+// a model's cd sets on the device: set c holds the states states[off[c] .. off[c+1]), combined by method (JB200_IWCD_*)
+struct CdSets { const int *off; const int *states; int method, nbest; };
+static __device__ float outprob_cd(const CdSets &cd, const float *__restrict__ row, int c) {
+  const int b0 = __ldg(cd.off + c), n_in = __ldg(cd.off + c + 1) - b0;
+  if (cd.method == JB200_IWCD_AVG) {
+    float sum = 0.0f; int j = 0;
+    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(cd.states + b0 + i)); if (v > JB200_LOG_ZERO) { sum += v; j++; } }
+    return sum / (float)j;
+  } else if (cd.method == JB200_IWCD_MAX) {
+    float mx = JB200_LOG_ZERO;
+    for (int i = 0; i < n_in; i++) { float v = __ldg(row + __ldg(cd.states + b0 + i)); if (mx < v) mx = v; }
+    return mx;
+  }
+  const int maxn = cd.nbest;
+  if (maxn <= 3) {
+    // the kept list is the sorted multiset of the maxn largest valid scores, and the result adds it up from the
+    // largest down (outprob.c:313-318): three registers instead of an indexed array in local memory
+    float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY; int n = 0;
+    for (int i = 0; i < n_in; i++) {
+      const float v = __ldg(row + __ldg(cd.states + b0 + i));
+      if (v <= JB200_LOG_ZERO) continue;
+      n++;
+      if (v > m0) { m2 = m1; m1 = m0; m0 = v; }
+      else if (v > m1) { m2 = m1; m1 = v; }
+      else if (v > m2) m2 = v;
+    }
+    n = min(n, maxn);
+    float prob = 0.0f;
+    if (n > 0) prob += m0;
+    if (n > 1) prob += m1;
+    if (n > 2) prob += m2;
+    return prob / (float)n;
+  }
+  float mp[NBEST_MAX + 1]; int n = 0;
+  for (int i = 0; i < n_in; i++) {
+    float prob = __ldg(row + __ldg(cd.states + b0 + i));
+    if (prob <= JB200_LOG_ZERO) continue;
+    if (n == 0 || prob <= mp[n - 1]) {
+      if (n == maxn) continue;
+      mp[n] = prob; n++;
+    } else {
+      for (int k = 0; k < n; k++) {
+        if (prob > mp[k]) {
+          int cnt = n - k - ((n == maxn) ? 1 : 0);
+          for (int q = k + cnt; q > k; q--) mp[q] = mp[q - 1];
+          mp[k] = prob;
+          break;
+        }
+      }
+      if (n < maxn) n++;
+    }
+  }
+  float prob = 0.0f;
+  for (int i = 0; i < n; i++) prob += mp[i];
+  return prob / (float)n;
+}
+
 // ---- DNN input splicing (wav2mfcc.c:160-183, splice_mfcc realtime-1stpass.c:445-460) -------------------------------
 // A DNN with context_len ctx > 1 takes frames fl = in_dim / ctx wide; network input row r is the concatenation of ctx
 // consecutive frames of a window.  A segment is an utterance of a batch or a stream's feed: its rows start at row0, and

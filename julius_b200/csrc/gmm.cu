@@ -4,7 +4,9 @@
 //   outprob_state -> calc_mix -> gprune_{none,safe,beam,heu} -> compute_g_base -> addlog_array
 //   (libsent/src/phmm/outprob.c:183-249, calc_mix.c:40-81, gprune_none.c:58-82,
 //    gprune_safe.c:75-202, gprune_common.c:41-126, addlog.c:102-123)
-// and for outprob_cd (outprob.c:286-400) in the cd-set kernel.
+// and for outprob_cd (outprob.c:286-400) in the cd-set kernel.  Where each rule lives: compute_g_base's exact distance in
+// gauss_dist_exact, the NULL-density rule in gauss_score (the pruned replay spells it out beside its give-up test),
+// addlog_array and calc_mix's finish in mix_add / mix_finish, outprob_cd in common.cuh (shared with the beam kernels).
 //
 // Layout in HBM.  One 16-byte aligned record per Gaussian, in quads so that a 64-bit register pair
 // holds two dimensions (a dimension pair is carried through the inner loop as one 64-bit value):
@@ -30,7 +32,6 @@ static constexpr int GMM_THREADS = 128;
 static constexpr int GMM_FPT = 2;              // frames per thread
 static constexpr int GMM_TILE_STATES = 4;      // max states per staged tile
 static constexpr int GMM_TILE_GAUSS = 64;      // max Gaussians per staged tile
-static constexpr int GMM_NMAX = 16;            // max -tmix for the pruned variants
 
 __host__ __device__ constexpr int gmm_stride(int D) { return ((2 * D + 2) + 3) & ~3; }
 
@@ -54,10 +55,39 @@ __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigne
   return pack2(__fmaf_rn(lo2(a), lo2(b), lo2(c)), __fmaf_rn(hi2(a), hi2(b), hi2(c)));
 }
 
-__device__ __forceinline__ float finish_exact(float lp) {
-  // calc_mix.c:72-80 for a single stream with weight 1
-  if (lp <= JB200_LOG_ZERO || lp == 0.0f) return JB200_LOG_ZERO;
-  return (float)((double)lp * JB200_INV_LOG_TEN);
+// compute_g_base's distance in the reference's fp32 statement order: gconst + sum over d of (x-m)*(x-m)*iv, no FMA
+// contraction.  The pruned K1 variants and the calcmix hook's per-Gaussian kernel use it; the unpruned variants run the
+// same formula paired (fma2) in the kernel.
+__device__ __forceinline__ float gauss_dist_exact(const float *rec, const float *x, int D) {
+  float acc = rec[rec_gconst(D)];
+#pragma unroll
+  for (int d = 0; d < D; d++) {
+    const float t = __fsub_rn(x[d], rec[rec_mean(d)]);
+    acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(t, t), rec[rec_ivar(d)]));
+  }
+  return acc;
+}
+
+// a Gaussian's log density from its distance; a NaN gconst marks a NULL density (gprune_none.c:66)
+__device__ __forceinline__ float gauss_score(float gconst, float acc) {
+  return (gconst != gconst) ? JB200_LOG_ZERO : acc * -0.5f;
+}
+
+// addlog_array (addlog.c:102-123) over a state's weighted mixture terms, fed from the last term down to the first:
+// adds the term sc to the running sum (y, ssum) and returns the new y.  The sum starts at addlog_array's seed, a term at
+// LOG_ZERO: y = LOG_ZERO, ssum = 1.  EXACT walks the table.  FAST keeps a streaming log-sum-exp, in which the seed
+// vanishes (expf underflows) unless every term lies within ~88 of LOG_ZERO, e.g. a state whose densities are all NULL.
+__device__ __forceinline__ float mix_add(bool exact, float y, float &ssum, float sc, const float *__restrict__ tbl) {
+  if (exact) return addlog_step_exact(y, sc, tbl);
+  if (sc > y) { ssum = ssum * __expf(y - sc) + 1.0f; return sc; }
+  ssum += __expf(sc - y);
+  return y;
+}
+// the state's score from the sum of its n terms, calc_mix.c:72-80 for a single stream with weight 1
+__device__ __forceinline__ float mix_finish(bool exact, float y, float ssum, int n) {
+  if (exact) return (y <= JB200_LOG_ZERO || y == 0.0f) ? JB200_LOG_ZERO : (float)((double)y * JB200_INV_LOG_TEN);
+  const float lp = y + __logf(ssum);
+  return (n == 0 || lp <= JB200_LOG_ZERO) ? JB200_LOG_ZERO : lp * (float)JB200_INV_LOG_TEN;
 }
 
 // cache_push, gprune_common.c:87-126 (score list sorted descending)
@@ -154,9 +184,7 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
       const int nm = mixcnt[tl.s0 + si];
       float res[GMM_FPT];
       if (!PRUNE) {
-        // streaming log-add from the LAST mixture down to the first (addlog.c:108-121)
-        // FAST: the running sum starts from addlog_array's seed, a term at LOG_ZERO (y = LOG_ZERO, ssum = 1).  It vanishes
-        // (expf underflows) unless every term lies within ~88 of LOG_ZERO, e.g. a state whose densities are all NULL
+        // mixtures from the LAST down to the first, as addlog_array adds them
         float y[GMM_FPT], ssum[GMM_FPT];
 #pragma unroll
         for (int k = 0; k < GMM_FPT; k++) { y[k] = JB200_LOG_ZERO; ssum[k] = 1.0f; }
@@ -192,61 +220,40 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
 #pragma unroll
             for (int k = 0; k < GMM_FPT; k++) acc[k] = ((D & 1) ? acc[k] : 0.0f) + lo2(acc2[k]) + hi2(acc2[k]);
           }
-          const bool invalid = (gconst != gconst);   // NaN marks a NULL density (gprune_none.c:66)
 #pragma unroll
           for (int k = 0; k < GMM_FPT; k++) {
-            float sc = invalid ? JB200_LOG_ZERO : acc[k] * -0.5f;
-            if (EXACT) {
-              sc = __fadd_rn(sc, lnw);
-              y[k] = addlog_step_exact(y[k], sc, tbl);
-            } else {
-              sc += lnw;
-              if (sc > y[k]) { ssum[k] = ssum[k] * __expf(y[k] - sc) + 1.0f; y[k] = sc; }
-              else ssum[k] += __expf(sc - y[k]);
-            }
+            const float sc = gauss_score(gconst, acc[k]);
+            y[k] = mix_add(EXACT, y[k], ssum[k], EXACT ? __fadd_rn(sc, lnw) : sc + lnw, tbl);
           }
         }
 #pragma unroll
-        for (int k = 0; k < GMM_FPT; k++) {
-          if (EXACT) res[k] = finish_exact(y[k]);
-          else {
-            float lp = y[k] + __logf(ssum[k]);
-            res[k] = (nm == 0 || lp <= JB200_LOG_ZERO) ? JB200_LOG_ZERO : lp * (float)JB200_INV_LOG_TEN;
-          }
-        }
+        for (int k = 0; k < GMM_FPT; k++) res[k] = mix_finish(EXACT, y[k], ssum[k], nm);
       } else {
         // safe pruning replay (gprune_safe.c:187-199): mixtures in index order, top-N list,
         // a candidate is dropped iff its full score <= current N-th best (early exit in
         // compute_g_safe is equivalent because the partial sums are non-decreasing).
 #pragma unroll
         for (int k = 0; k < GMM_FPT; k++) {
-          float cs[GMM_NMAX]; int ci[GMM_NMAX];
+          float cs[NBEST_MAX]; int ci[NBEST_MAX];
           int num = 0; float thres = JB200_LOG_ZERO;
           for (int m = 0; m < nm; m++) {
             const float *rec = pb + (size_t)(grel + m) * STRIDE;
             const float gconst = rec[rec_gconst(D)];
-            float acc = gconst;
-#pragma unroll
-            for (int d = 0; d < D; d++) {
-              float x = __fsub_rn(v[k][d], rec[rec_mean(d)]);
-              acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(x, x), rec[rec_ivar(d)]));
-            }
+            const float acc = gauss_dist_exact(rec, v[k], D);
             // compute_g_safe gives up (LOG_ZERO) as soon as its partial sum passes thres * -2; the partial sums never
             // decrease, so that is the full sum passing it.  Such a LOG_ZERO is kept when thres itself is below LOG_ZERO.
+            // This is gauss_score with the give-up test between its two cases; tested after it, the compiler gives
+            // these kernels more registers.
             float sc = (gconst != gconst) ? JB200_LOG_ZERO
                      : (num >= gprune_num && acc > thres * -2.0f) ? JB200_LOG_ZERO : acc * -0.5f;
             if (num >= gprune_num && sc <= thres) continue;
             num = cache_push_dev(cs, ci, gprune_num, m, sc, num);
             thres = cs[num - 1];
           }
-          float y = JB200_LOG_ZERO, ssum = 1.0f;   // seeded as above
-          for (int i = num - 1; i >= 0; i--) {
-            float sc = __fadd_rn(cs[i], pb[(size_t)(grel + ci[i]) * STRIDE + rec_lnw(D)]);
-            if (EXACT) y = addlog_step_exact(y, sc, tbl);
-            else { if (sc > y) { ssum = ssum * __expf(y - sc) + 1.0f; y = sc; } else ssum += __expf(sc - y); }
-          }
-          if (EXACT) res[k] = finish_exact(y);
-          else { float lp = y + __logf(ssum); res[k] = (num == 0 || lp <= JB200_LOG_ZERO) ? JB200_LOG_ZERO : lp * (float)JB200_INV_LOG_TEN; }
+          float y = JB200_LOG_ZERO, ssum = 1.0f;
+          for (int i = num - 1; i >= 0; i--)
+            y = mix_add(EXACT, y, ssum, __fadd_rn(cs[i], pb[(size_t)(grel + ci[i]) * STRIDE + rec_lnw(D)]), tbl);
+          res[k] = mix_finish(EXACT, y, ssum, num);
         }
       }
 #pragma unroll
@@ -260,47 +267,11 @@ gmm_score_kernel(const float *__restrict__ pk, const GmmTile *__restrict__ tiles
 
 // ---- pseudo-phone set scores (outprob.c:286-400) -------------------------------------------
 __global__ void __launch_bounds__(256)
-cdset_kernel(float *__restrict__ rows, int T, int row_stride, int S, int C,
-             const int *__restrict__ cd_off, const int *__restrict__ cd_states, int method, int maxn) {
+cdset_kernel(float *__restrict__ rows, int T, int row_stride, int S, int C, CdSets cd) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y;
   if (c >= C || t >= T) return;
-  const float *st = rows + (size_t)t * row_stride;
-  const int b0 = cd_off[c], n_in = cd_off[c + 1] - b0;
-  float out;
-  if (method == JB200_IWCD_AVG) {
-    float sum = 0.0f; int j = 0;
-    for (int i = 0; i < n_in; i++) { float p = st[cd_states[b0 + i]]; if (p > JB200_LOG_ZERO) { sum = __fadd_rn(sum, p); j++; } }
-    out = __fdiv_rn(sum, (float)j);
-  } else if (method == JB200_IWCD_MAX) {
-    float mx = JB200_LOG_ZERO;
-    for (int i = 0; i < n_in; i++) { float p = st[cd_states[b0 + i]]; if (mx < p) mx = p; }
-    out = mx;
-  } else {
-    float mp[GMM_NMAX + 1]; int n = 0;
-    for (int i = 0; i < n_in; i++) {
-      float prob = st[cd_states[b0 + i]];
-      if (prob <= JB200_LOG_ZERO) continue;
-      if (n == 0 || prob <= mp[n - 1]) {
-        if (n == maxn) continue;
-        mp[n] = prob; n++;
-      } else {
-        for (int k = 0; k < n; k++) {
-          if (prob > mp[k]) {
-            int cnt = n - k - ((n == maxn) ? 1 : 0);
-            for (int q = k + cnt; q > k; q--) mp[q] = mp[q - 1];
-            mp[k] = prob;
-            break;
-          }
-        }
-        if (n < maxn) n++;
-      }
-    }
-    float prob = 0.0f;
-    for (int i = 0; i < n; i++) prob = __fadd_rn(prob, mp[i]);
-    out = __fdiv_rn(prob, (float)n);
-  }
-  rows[(size_t)t * row_stride + S + c] = out;
+  rows[(size_t)t * row_stride + S + c] = outprob_cd(cd, rows + (size_t)t * row_stride, c);
 }
 
 // ---- per-Gaussian scores of one frame (calcmix hook contract) ----------------------------------
@@ -309,13 +280,7 @@ __global__ void gauss_frame_kernel(const float *__restrict__ pk, int stride, int
   int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= G) return;
   const float *rec = pk + (size_t)g * stride;
-  float gconst = rec[rec_gconst(D)];
-  float acc = gconst;
-  for (int d = 0; d < D; d++) {
-    float x = __fsub_rn(feat[d], rec[rec_mean(d)]);
-    acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(x, x), rec[rec_ivar(d)]));
-  }
-  out[g] = (gconst != gconst) ? JB200_LOG_ZERO : acc * -0.5f;
+  out[g] = gauss_score(rec[rec_gconst(D)], gauss_dist_exact(rec, feat, D));
 }
 
 }  // namespace jb200
@@ -335,6 +300,7 @@ struct jb200_gmm {
   cudaStream_t stream = nullptr;
   // scratch for the host variants
   float *d_feats = nullptr, *d_rows = nullptr; size_t cap_frames = 0;
+  float *d_gfeat = nullptr, *d_gauss = nullptr;   // jb200_gmm_gauss_host: one frame in, G Gaussian scores out
   int sm_count = 132;
 };
 
@@ -342,17 +308,14 @@ namespace jb200 {
 int gmm_device(const jb200_gmm *h) { return h->device; }
 cudaStream_t gmm_stream(const jb200_gmm *h) { return h->stream; }
 int gmm_dim(const jb200_gmm *h) { return h->D; }
-int gmm_cd_device(const jb200_gmm *h, const int **cd_off, const int **cd_states, int *method, int *nbest) {
-  *cd_off = h->d_cd_off; *cd_states = h->d_cd_states; *method = h->iwcd_method; *nbest = h->iwcd_nbest;
-  return 0;
-}
+CdSets gmm_cdsets(const jb200_gmm *h) { return {h->d_cd_off, h->d_cd_states, h->iwcd_method, h->iwcd_nbest}; }
 }
 
 extern "C" void jb200_gmm_destroy(jb200_gmm *h) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaFree(h->d_pk); cudaFree(h->d_tiles); cudaFree(h->d_cd_off); cudaFree(h->d_cd_states); cudaFree(h->d_tbl);
-  cudaFree(h->d_feats); cudaFree(h->d_rows);
+  cudaFree(h->d_feats); cudaFree(h->d_rows); cudaFree(h->d_gfeat); cudaFree(h->d_gauss);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -402,15 +365,17 @@ static int gmm_build(jb200_gmm *h, const jb200_gmm_desc *d, const std::vector<in
   build_addlog_table(tbl);
   JB_CUDA(cudaMalloc(&h->d_tbl, tbl.size() * sizeof(float)));
   JB_CUDA(cudaMemcpy(h->d_tbl, tbl.data(), tbl.size() * sizeof(float), cudaMemcpyHostToDevice));
+  JB_CUDA(cudaMalloc(&h->d_gfeat, sizeof(float) * h->D));
+  JB_CUDA(cudaMalloc(&h->d_gauss, sizeof(float) * (h->G + 1)));
   return JB200_OK;
 }
 
 extern "C" int jb200_gmm_create(const jb200_gmm_desc *d, int device, int mode, jb200_gmm **out) {
   if (!d || !out) { set_error("jb200_gmm_create: null argument"); return JB200_ERR_ARG; }
-  if (d->gprune_method != JB200_GPRUNE_NONE && (d->gprune_num < 1 || d->gprune_num > GMM_NMAX)) {
-    set_error("-tmix %d outside supported range 1..%d", d->gprune_num, GMM_NMAX); return JB200_ERR_UNSUPPORTED;
+  if (d->gprune_method != JB200_GPRUNE_NONE && (d->gprune_num < 1 || d->gprune_num > NBEST_MAX)) {
+    set_error("-tmix %d outside supported range 1..%d", d->gprune_num, NBEST_MAX); return JB200_ERR_UNSUPPORTED;
   }
-  if (d->iwcd_method == JB200_IWCD_NBEST && d->iwcd_nbest > GMM_NMAX) { set_error("-iwcd1 best %d too large", d->iwcd_nbest); return JB200_ERR_UNSUPPORTED; }
+  if (d->iwcd_method == JB200_IWCD_NBEST && d->iwcd_nbest > NBEST_MAX) { set_error("-iwcd1 best %d too large", d->iwcd_nbest); return JB200_ERR_UNSUPPORTED; }
   if (d->n_gauss > 0 && d->dim != 39 && d->dim != 38 && d->dim != 26 && d->dim != 25) {
     set_error("feature dimension %d not instantiated (39, 38, 26, 25)", d->dim); return JB200_ERR_UNSUPPORTED;
   }
@@ -477,8 +442,7 @@ extern "C" int jb200_gmm_cdsets_device(jb200_gmm *h, float *d_rows, int T, void 
   for (int t0 = 0; t0 < T; t0 += 65535) {
     int tt = T - t0 < 65535 ? T - t0 : 65535;
     dim3 grid((h->C + 255) / 256, tt);
-    cdset_kernel<<<grid, 256, 0, st>>>(d_rows + (size_t)t0 * h->row_stride, tt, h->row_stride, h->S, h->C, h->d_cd_off, h->d_cd_states,
-                                       h->iwcd_method, h->iwcd_nbest);
+    cdset_kernel<<<grid, 256, 0, st>>>(d_rows + (size_t)t0 * h->row_stride, tt, h->row_stride, h->S, h->C, gmm_cdsets(h));
     JB_LAUNCH_CHECK();
   }
   return JB200_OK;
@@ -520,42 +484,36 @@ static int ensure_scratch(jb200_gmm *h, int T) {
   return JB200_OK;
 }
 
-extern "C" int jb200_gmm_score_rows_host(jb200_gmm *h, const float *feats, int T, float *rows) {
-  if (!h || !feats || !rows) { set_error("jb200_gmm_score_rows_host: null argument"); return JB200_ERR_ARG; }
+// uploads T frames, scores them into the scratch rows and copies the first cols columns of each row back, cols apart
+static int score_host(jb200_gmm *h, const float *feats, int T, float *out, int cols) {
   if (T <= 0) return JB200_OK;
   JB_CUDA(cudaSetDevice(h->device));
-  int rc = ensure_scratch(h, T); if (rc) return rc;
+  JB_RC(ensure_scratch(h, T));
   JB_CUDA(cudaMemcpyAsync(h->d_feats, feats, (size_t)T * h->D * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  rc = jb200_gmm_score_device(h, h->d_feats, T, h->d_rows, h->stream); if (rc) return rc;
-  JB_CUDA(cudaMemcpyAsync(rows, h->d_rows, (size_t)T * h->row_stride * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  JB_RC(jb200_gmm_score_device(h, h->d_feats, T, h->d_rows, h->stream));
+  JB_CUDA(cudaMemcpy2DAsync(out, (size_t)cols * sizeof(float), h->d_rows, (size_t)h->row_stride * sizeof(float),
+                            (size_t)cols * sizeof(float), T, cudaMemcpyDeviceToHost, h->stream));
   JB_CUDA(cudaStreamSynchronize(h->stream));
   return JB200_OK;
 }
 
+extern "C" int jb200_gmm_score_rows_host(jb200_gmm *h, const float *feats, int T, float *rows) {
+  if (!h || !feats || !rows) { set_error("jb200_gmm_score_rows_host: null argument"); return JB200_ERR_ARG; }
+  return score_host(h, feats, T, rows, h->row_stride);
+}
+
 extern "C" int jb200_gmm_score_host(jb200_gmm *h, const float *feats, int T, float *scores) {
   if (!h || !feats || !scores) { set_error("jb200_gmm_score_host: null argument"); return JB200_ERR_ARG; }
-  if (T <= 0) return JB200_OK;
-  JB_CUDA(cudaSetDevice(h->device));
-  int rc = ensure_scratch(h, T); if (rc) return rc;
-  JB_CUDA(cudaMemcpyAsync(h->d_feats, feats, (size_t)T * h->D * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  rc = jb200_gmm_score_device(h, h->d_feats, T, h->d_rows, h->stream); if (rc) return rc;
-  JB_CUDA(cudaMemcpy2DAsync(scores, (size_t)h->S * sizeof(float), h->d_rows, (size_t)h->row_stride * sizeof(float),
-                            (size_t)h->S * sizeof(float), T, cudaMemcpyDeviceToHost, h->stream));
-  JB_CUDA(cudaStreamSynchronize(h->stream));
-  return JB200_OK;
+  return score_host(h, feats, T, scores, h->S);
 }
 
 extern "C" int jb200_gmm_gauss_host(jb200_gmm *h, const float *feat, float *gauss) {
   if (!h || !feat || !gauss) { set_error("jb200_gmm_gauss_host: null argument"); return JB200_ERR_ARG; }
   JB_CUDA(cudaSetDevice(h->device));
-  float *d_f = nullptr, *d_o = nullptr;
-  JB_CUDA(cudaMalloc(&d_f, sizeof(float) * h->D));
-  JB_CUDA(cudaMalloc(&d_o, sizeof(float) * (h->G + 1)));
-  JB_CUDA(cudaMemcpyAsync(d_f, feat, sizeof(float) * h->D, cudaMemcpyHostToDevice, h->stream));
-  gauss_frame_kernel<<<(h->G + 255) / 256, 256, 0, h->stream>>>(h->d_pk, h->stride, h->D, h->G, d_f, d_o);
+  JB_CUDA(cudaMemcpyAsync(h->d_gfeat, feat, sizeof(float) * h->D, cudaMemcpyHostToDevice, h->stream));
+  gauss_frame_kernel<<<(h->G + 255) / 256, 256, 0, h->stream>>>(h->d_pk, h->stride, h->D, h->G, h->d_gfeat, h->d_gauss);
   JB_LAUNCH_CHECK();
-  JB_CUDA(cudaMemcpyAsync(gauss, d_o, sizeof(float) * h->G, cudaMemcpyDeviceToHost, h->stream));
+  JB_CUDA(cudaMemcpyAsync(gauss, h->d_gauss, sizeof(float) * h->G, cudaMemcpyDeviceToHost, h->stream));
   JB_CUDA(cudaStreamSynchronize(h->stream));
-  cudaFree(d_f); cudaFree(d_o);
   return JB200_OK;
 }
